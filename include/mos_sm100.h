@@ -1,4 +1,4 @@
-/* mos_sm100.h — C ABI of libmos_sm100.so, the B200 (sm_100a) ED-LoRA diffusion hot path.
+/* mos_sm100.h — C ABI of libmos_sm100.so, the H100 (sm_90a) ED-LoRA diffusion hot path (the names are historical).
  *
  * Conventions (SURVEY.md §8b): every entry point returns int (0 = ok, negative = MOS_E*); the message of the
  * last failure on the calling thread is available from mos_last_error(). All pointers are raw device pointers
@@ -6,7 +6,7 @@
  * pointer after return and never synchronises: work is enqueued on the cudaStream_t passed as `stream`.
  * Activations and packed weights are 16-bit, NHWC / token-major resp. K-major: bf16 (training) or fp16 (sampling: the
  * reference's own sampling precision; its three extra mantissa bits keep the classifier-free-guidance difference accurate,
- * DESIGN.md "numerics"); `act_dtype` / MOS_DT_* selects the type.  tcgen05 kind::f16 takes ONE operand format per MMA, so
+ * DESIGN.md "numerics"); `act_dtype` / MOS_DT_* selects the type.  wgmma takes ONE operand type for A and B, so
  * the operands of a GEMM share the type.  Accumulation, statistics and softmax are fp32.
  *
  * Each entry point cites the reference call site it replaces (paths relative to TencentARC/Mix-of-Show).
@@ -30,7 +30,7 @@ const char* mos_last_error(void);
 /* ------------------------------------------------------------------------------------------------------------
  * Fused GEMM (+ implicit-GEMM 3x3 convolution) with LoRA / bias / temb / GEGLU / residual epilogue.
  *   out[m, n] = epi( sum_k A[m, k] * W[n, k]  +  sum_r (sum_k A[m,k] * lora_down[r,k]) * lora_up[n, r] )
- * Replaces, in one tcgen05 kernel:
+ * Replaces, in one wgmma kernel:
  *   - LoRALinearLayer.forward                     mixofshow/models/edlora.py:244-246
  *   - attn.to_q / to_k / to_v / to_out[0]         mixofshow/models/edlora.py:143-145,161 (and :69-71,88)
  *   - region to_k / to_v                          mixofshow/pipelines/pipeline_regionally_t2iadapter.py:122-126
@@ -74,9 +74,8 @@ typedef struct mos_gemm_args {
   int32_t w_static;       /* reserved, ignored (round 1 requested the first W tiles ahead of griddepcontrol.wait when set; the
                            * measurement was neutral and the path was removed) */
   int32_t a_dtype;        /* MOS_DT_*: type of A, of the 16-bit outputs (rows, head-split) and of `residual` */
-  int32_t w_dtype;        /* MOS_DT_*: type of W and lora_down; must equal a_dtype (one operand format per tcgen05 MMA) */
-  int32_t pair_mode;      /* 0 = library heuristic, 1 = force 2-CTA pair tiles (needs an even number of 128-row tiles),
-                           * 2 = force the 1-CTA kernel (benchmarking) */
+  int32_t w_dtype;        /* MOS_DT_*: type of W and lora_down; must equal a_dtype (one operand type per wgmma) */
+  int32_t pair_mode;      /* reserved, ignored: every launch runs 128 x 160 tiles of one CTA */
   int32_t* tile_counters; /* split-K only, optional: int32 [tile_counters_len] device counters, ZERO on entry (the kernel
                            * leaves them zero).  When given, the launch also finalizes: the `splits` CTAs of an output tile
                            * sum the partials in split order and write bias / bias_batch / residual -> `out` themselves
@@ -95,19 +94,13 @@ int mos_gemm_bf16(const mos_gemm_args* args, void* stream);
  * prefetch done, accumulators ready, accumulators drained, tile written]. */
 int mos_debug_set_timeline(void* buf);
 
-/* Profiling aid for mos_attention_fwd: register a device buffer of 256 uint64 (or NULL to disable); CTA (0,0) of every
- * subsequent launch stores clock64 stamps for its first 32 kv tiles: softmax warp 0 at [j*4 + k] (k: before s_full wait,
- * S visible, softmax pass done, P published) and the MMA thread at [128 + j*4 + k] (k: K/V landed, S buffer free and
- * S_j issued next, before p_full wait, P visible and PV_j issued next). */
-int mos_debug_set_attn_timeline(void* buf);
-
 /* Sum split-K partials and apply bias / bias_batch / residual -> bf16 [M, ldc]. */
 int mos_splitk_finalize(const float* partial, int32_t splits, int64_t M, int64_t N, const float* bias,
                         const float* bias_batch, int64_t rows_per_batch, int64_t bias_batch_ld,
                         const void* residual, int64_t ldr, void* out, int64_t ldc, int32_t act_dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Flash attention (tcgen05 S = QK^T and PV in TMEM, online softmax in registers), head_dim in {40, 80, 160}.
+ * Flash attention (wgmma S = QK^T and PV, accumulators and online softmax in registers), head_dim in {40, 80, 160}.
  *   Q, K : bf16 [batch*heads, nq|nk, DP]   DP = head_dim rounded up to 64, pad columns zero
  *   Vt   : bf16 [batch*heads, DV, nk8]     DV = head_dim rounded up to 16, nk8 = nk rounded up to 8, pads zero
  *   out  : bf16 [batch, nq, ldo], head h at columns [h*head_dim, (h+1)*head_dim)

@@ -1,28 +1,17 @@
-// attention.cu — K2/K3: flash attention on tcgen05 for the SD1.5 head sizes d = 40 / 80 / 160 (8 heads).
+// attention.cu — K2/K3: flash attention on wgmma (sm_90a) for the SD1.5 head sizes d = 40 / 80 / 160 (8 heads).
 //
 //   O = softmax(Q K^T * scale) V     per (batch, head);  self-attention (N x N) and cross-attention (N x 77)
 //
 // Replaces xformers.ops.memory_efficient_attention / attn.get_attention_scores + bmm at
 // mixofshow/models/edlora.py:77-83,151-156 and pipeline_regionally_t2iadapter.py:111-116.
 //
-// One CTA = one 128-query tile of one (batch, head).  192 threads:
-//   warps 0..3  softmax: one thread owns one query row.  tcgen05.ld S from TMEM ONCE per tile, p = 2^(s*c - m_ref)
-//               against a lazily updated reference maximum, P -> bf16 -> 128B-swizzled smem
-//   warp 4      TMA producer (Q once, K / V^T ring)
-//   warp 5      TMEM allocator + tcgen05.mma issuer: S_j = Q K_j^T (TMEM), O += P_j V_j (one TMEM accumulator)
-// Design notes (measurements in profiles/README.md):
-//   * lazy reference maximum: tile j is exponentiated against the running maximum of tiles < j (exact: softmax is shift
-//     invariant; p <= 2^32 is harmless in fp32 / bf16).  Only tile 0 takes a row-max pre-pass; a tile whose maximum
-//     exceeds the reference by more than 2^32 is redone against its own maximum (warp-uniform slow path).  The reference
-//     only moves when a tile maximum exceeds it by more than 8 (log2 units), so rescales are rare.
-//   * PV_j accumulates into ONE TMEM accumulator (tcgen05.mma accumulate flag); when the reference moved, the owning
-//     thread rescales its O row in TMEM (tcgen05.ld / tcgen05.st) before it publishes P_j.  O is read once, at the end.
-//   * d = 40 self-attention: 64-key tiles with S and P double buffered, a 3-stage K/V ring, 256 TMEM columns and 91 KB of
-//     smem, so that two CTAs share an SM and neither waits for S_{j+1} or for the P buffer.
-//   * full tiles run a straight-line pass (no per-chunk branches: instruction-fetch bubbles after branches were 11 % of
-//     the issue-stall samples), 4 independent max / sum accumulators, TMEM loads one 16-column chunk ahead.
+// One CTA = one 128-query tile of one (batch, head).  288 threads:
+//   warps 0..7  two consumer warpgroups, 64 query rows each: S_j = Q K_j^T (wgmma, A and B from shared memory) into
+//               registers, online softmax in registers (a row lives in the 4 lanes of a quad), P_j packed to 16 bits in
+//               registers and fed back as the A operand of O += P_j V_j (wgmma, A from registers); O stays in registers
+//   warp 8      TMA producer (Q once, K / V^T ring)
 // Layouts (written by the QKV GEMM epilogue): Q,K [B*H, rows, DP] (DP = d padded to 64, pad = 0),
-// V^T [B*H, DV, nk8] (keys contiguous), so every MMA operand is K-major SWIZZLE_128B.
+// V^T [B*H, DV, nk8] (keys contiguous), so every shared-memory operand is K-major SWIZZLE_128B.
 #include <stdlib.h>
 
 #include "common.h"
@@ -45,225 +34,72 @@ struct AttnDev {
   float* lse2;   // optional [B*H, nq]: log2-domain log-sum-exp of scale*S (saved for the backward kernels)
   float* pcols;  // optional [B*H, nq, 2]: probabilities at key columns pos[b][0..1] (single kv tile only)
   const int* pos;
-  unsigned long long* tl;   // timeline buffer of the TL instantiation (mos_debug_set_attn_timeline)
 };
 
-// ONE: single-tile variant for cross-attention (nk <= 128): one 128-key tile, nothing double buffered, so that the
-// probability maps / concept-token columns of the controller and regulariser paths come from a single kv tile.
+constexpr int ATTN_THREADS = 256 + 32;   // two consumer warpgroups + the TMA producer warp
+
+// ONE: single-tile variant for cross-attention (nk <= 128): one 128-key tile, so that the probability maps /
+// concept-token columns of the controller and regulariser paths come from a single kv tile.
 template <int D, bool ONE = false>
 struct AttnCfg {
   static constexpr int KSTEPS = (D + 15) / 16;
   static constexpr int DP = ((D + 63) / 64) * 64;
   static constexpr int QCH = DP / 64;
   static constexpr int DV = ((D + 15) / 16) * 16;
-  static constexpr int BKV = ONE ? 128 : (D <= 40 ? 64 : (D <= 80 ? 128 : 64));
+  static constexpr int BKV = ONE ? 128 : (D <= 80 ? 128 : 64);
   static constexpr int KVCH = BKV / 64;
-  static constexpr int STAGES = ONE ? 1 : (D <= 40 ? 3 : 2);
-  static constexpr int SB = ONE ? 1 : 2;
-  static constexpr int PB = ONE ? 1 : 2;
-  static constexpr int MINB = D <= 40 ? 2 : 1;
+  static constexpr int STAGES = ONE ? 1 : 2;
   static constexpr int Q_BYTES = QCH * 128 * 128;
   static constexpr int K_BYTES = QCH * BKV * 128;
   static constexpr int V_BYTES = KVCH * DV * 128;
-  static constexpr int P_BYTES = KVCH * 128 * 128;
-  static constexpr int O_COL0 = SB * BKV;
-  static constexpr int TMEM_COLS = (O_COL0 + DV <= 256) ? 256 : 512;
-  static constexpr int SMEM_BYTES = Q_BYTES + STAGES * (K_BYTES + V_BYTES) + PB * P_BYTES + 1024;
-  static_assert(O_COL0 + DV <= TMEM_COLS, "TMEM budget");
-  static_assert(MINB * SMEM_BYTES <= 227 * 1024, "smem budget");
+  static constexpr int SMEM_BYTES = Q_BYTES + STAGES * (K_BYTES + V_BYTES) + 1024;
+  static_assert(SMEM_BYTES <= 227 * 1024, "smem budget");
 };
 
-// 16 logits of one row -> probabilities (fp32 sums, running raw maxima, packed bf16 pairs)
-template <bool WHOLE, bool PC, bool F16>
-__device__ __forceinline__ void s_chunk(const uint32_t (&v)[16], int col0, int kv_valid, float c, float nm,
-                                        float (&s4)[4], float (&m4)[4], uint32_t (&pk)[8], int pos0, int pos1,
-                                        float& pc0, float& pc1) {
-#pragma unroll
-  for (int i = 0; i < 16; i += 2) {
-    const float x0 = __uint_as_float(v[i]), x1 = __uint_as_float(v[i + 1]);
-    float e0 = ex2_approx(fmaf(x0, c, nm)), e1 = ex2_approx(fmaf(x1, c, nm));
-    if (WHOLE) {
-      m4[i & 3] = fmaxf(m4[i & 3], x0);
-      m4[(i + 1) & 3] = fmaxf(m4[(i + 1) & 3], x1);
-    } else {
-      const bool ok0 = col0 + i < kv_valid, ok1 = col0 + i + 1 < kv_valid;
-      m4[i & 3] = ok0 ? fmaxf(m4[i & 3], x0) : m4[i & 3];
-      m4[(i + 1) & 3] = ok1 ? fmaxf(m4[(i + 1) & 3], x1) : m4[(i + 1) & 3];
-      e0 = ok0 ? e0 : 0.f;
-      e1 = ok1 ? e1 : 0.f;
-    }
-    s4[i & 3] += e0;
-    s4[(i + 1) & 3] += e1;
-    if (PC) {
-      pc0 = (col0 + i == pos0) ? e0 : pc0;
-      pc0 = (col0 + i + 1 == pos0) ? e1 : pc0;
-      pc1 = (col0 + i == pos1) ? e0 : pc1;
-      pc1 = (col0 + i + 1 == pos1) ? e1 : pc1;
-    }
-    pk[i >> 1] = pack16x2<F16>(e0, e1);
-  }
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
-// row maximum of one S tile (raw logits), masked to the first kv_valid columns
-template <int BKV>
-__device__ __forceinline__ float s_row_max(uint32_t ts, int kv_valid, int row_lim) {
-  constexpr int NCH = BKV / 16;
-  uint32_t v[2][16];
-  float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-  tmem_ld16(ts, v[0]);
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    if (ch * 16 >= kv_valid) break;
-    tmem_ld_wait();
-    if (ch + 1 < NCH && (ch + 1) * 16 < kv_valid) tmem_ld16(ts + (ch + 1) * 16, v[(ch + 1) & 1]);
-    // row_lim <= kv_valid: columns this row may attend to (== kv_valid unless the launch is causal); the branch is
-    // taken per lane, the loads above are warp-uniform
-    if ((ch + 1) * 16 <= row_lim) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(v[ch & 1][i]));
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (ch * 16 + i < row_lim) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(v[ch & 1][i]));
-    }
-  }
-  return fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-}
-
-// the P buffer is free once PV_{j-PB} has retired; one lane polls
-__device__ __forceinline__ void wait_p_empty(uint64_t* bar, uint32_t parity, int lane) {
-  if (lane == 0) mbar_wait(bar, parity);
-  __syncwarp();
-}
-
-// Straight-line pass over a FULL S tile: p = 2^(s * c - m_ref) -> bf16 -> swizzled smem; row sum and raw row maximum.
-// TMEM loads are 32 columns wide and run one load ahead (a tcgen05.ld takes ~300 cycles to return while the tensor pipe
-// is busy, about the time the arithmetic of 32 columns needs); no branches besides the (normally already satisfied)
-// P-buffer wait.
-template <int BKV, bool F16>
-__device__ __forceinline__ void s_softmax_pass_full(uint32_t ts, float c, float m_ref, uint32_t sPb, int r,
-                                                    uint64_t* p_empty_bar, uint32_t pe_parity, int lane, float& rs,
-                                                    float& mx) {
-  constexpr int NCH = BKV / 32;
-  uint32_t v[2][32];
-  float s4[4] = {0.f, 0.f, 0.f, 0.f};
-  float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-  const float nm = -m_ref;
-  float unused0 = 0.f, unused1 = 0.f;
-  tmem_ld32(ts, v[0]);
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    tmem_ld_wait();
-    if (ch + 1 < NCH) tmem_ld32(ts + (ch + 1) * 32, v[(ch + 1) & 1]);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t pk[8];
-      const uint32_t(&vh)[16] = *reinterpret_cast<const uint32_t(*)[16]>(&v[ch & 1][h * 16]);
-      s_chunk<true, false, F16>(vh, ch * 32 + h * 16, BKV, c, nm, s4, m4, pk, -1, -1, unused0, unused1);
-      if (ch == 0 && h == 0) wait_p_empty(p_empty_bar, pe_parity, lane);
-      const int c16b = ch * 2 + h;        // 16-column chunk index inside the tile
-      const uint32_t rowp = sPb + (c16b >> 2) * 16384 + r * 128;
-#pragma unroll
-      for (int g = 0; g < 2; ++g) {
-        const int c16 = (c16b & 3) * 2 + g;  // 16-byte chunk inside the 128-byte row
-        sts128(rowp + ((c16 ^ (r & 7)) << 4), pk[g * 4 + 0], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
-      }
-    }
-  }
-  rs = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-  mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-}
-
-// General pass (partial tiles, concept-token columns, causal rows, redo path): masks the columns >= row_lim
-// (row_lim == kv_valid unless the launch is causal; chunks >= kv_valid are skipped by the whole warp).
-template <int BKV, bool PC, bool F16>
-__device__ __noinline__ void s_softmax_pass(uint32_t ts, float c, float m_ref, int kv_valid, int row_lim, uint32_t sPb, int r,
-                                            uint64_t* p_empty_bar, uint32_t pe_parity, bool wait_pe, int lane,
-                                            float& rs, float& mx, int pos0, int pos1, float& pc0, float& pc1) {
-  constexpr int NCH = BKV / 16;
-  uint32_t v[2][16];
-  float s4[4] = {0.f, 0.f, 0.f, 0.f};
-  float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-  const float nm = -m_ref;
-  tmem_ld16(ts, v[0]);
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    if (ch * 16 >= kv_valid) break;       // warp-uniform: whole chunk masked (PV reads only ceil(kv_valid / 16) k-steps)
-    tmem_ld_wait();
-    if (ch + 1 < NCH && (ch + 1) * 16 < kv_valid) tmem_ld16(ts + (ch + 1) * 16, v[(ch + 1) & 1]);
-    uint32_t pk[8];
-    s_chunk<false, PC, F16>(v[ch & 1], ch * 16, row_lim, c, nm, s4, m4, pk, pos0, pos1, pc0, pc1);
-    if (ch == 0 && wait_pe) wait_p_empty(p_empty_bar, pe_parity, lane);
-    const uint32_t rowp = sPb + (ch >> 2) * 16384 + r * 128;
-#pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      const int c16 = (ch & 3) * 2 + g;
-      sts128(rowp + ((c16 ^ (r & 7)) << 4), pk[g * 4 + 0], pk[g * 4 + 1], pk[g * 4 + 2], pk[g * 4 + 3]);
-    }
-  }
-  rs = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-  mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-}
-
-// optional in-kernel timeline (TL instantiation only, mos_debug_set_attn_timeline): CTA (0,0) records clock64 stamps of
-// its softmax warp 0 (role 0) and of the MMA thread (role 1) for the first 32 kv tiles, 4 stamps per tile and role.
-#define astamp(role, j, k)                                                                                     \
-  do {                                                                                                         \
-    if (TL && blockIdx.x == 0 && blockIdx.y == 0 && (j) < 32) p.tl[(role) * 128 + (j) * 4 + (k)] = clock64();  \
-  } while (0)
-
-template <int D, bool ONE, bool TL, bool CAUSAL = false, bool F16 = false>
-__global__ void __launch_bounds__(192, AttnCfg<D, ONE>::MINB)
+template <int D, bool ONE, bool CAUSAL = false, bool F16 = false>
+__global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
             const __grid_constant__ CUtensorMap tmV, const AttnDev p) {
   using C = AttnCfg<D, ONE>;
+  constexpr int NS = C::BKV / 2;    // S fragment registers per thread
+  constexpr int NO = C::DV / 2;     // O fragment registers per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sKV = sQ + C::Q_BYTES;
-  uint8_t* sP = sKV + C::STAGES * (C::K_BYTES + C::V_BYTES);
 
   __shared__ uint64_t q_full, kv_full[C::STAGES], kv_empty[C::STAGES];
-  __shared__ uint64_t s_full[2], s_empty[2], p_full[2], p_empty[2], o_full, o_done;
-  __shared__ uint32_t tmem_holder;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
   const int T = (p.nk + C::BKV - 1) / C::BKV;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(&q_full, 1);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
+      mbar_init(&kv_empty[s], 8);     // one arrival per consumer warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&s_full[s], 1);
-      mbar_init(&s_empty[s], 4);     // one arrival per softmax warp (lane 0, after __syncwarp)
-      mbar_init(&p_full[s], 4);
-      mbar_init(&p_empty[s], 1);
-    }
-    mbar_init(&o_full, 1);
-    mbar_init(&o_done, 1);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(&tmem_holder, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_holder;
   pdl_wait();               // Q / K / V^T come from the previous kernel in the stream
   pdl_launch_dependents();
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================================================================= TMA producer
     if (lane == 0) {
       mbar_expect_tx(&q_full, C::Q_BYTES);
@@ -272,7 +108,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
       int st = 0;
       uint32_t ph = 0;
       for (int j = 0; j < T; ++j) {
-        mbar_wait_hint(&kv_empty[st], ph ^ 1);     // long waits: park instead of polling next to the softmax warps
+        mbar_wait_hint(&kv_empty[st], ph ^ 1);
         uint8_t* sK = sKV + st * (C::K_BYTES + C::V_BYTES);
         uint8_t* sV = sK + C::K_BYTES;
         mbar_expect_tx(&kv_full[st], C::K_BYTES + C::V_BYTES);
@@ -288,210 +124,153 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================================================= MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc(128, C::BKV, F16 ? 0 : 1);
-      const uint32_t idesc_o = make_idesc(128, C::DV, F16 ? 0 : 1);
-      mbar_wait(&q_full, 0);
-      int st_s = 0, st_p = 0;          // K/V ring slot of the next S product / of the next PV product
-      uint32_t ph_s = 0;
-      for (int j = 0; j <= T; ++j) {
-        if (j < T) {
-          const int sb = j % C::SB;
-          mbar_wait(&kv_full[st_s], ph_s);
-          astamp(1, j, 0);
-          mbar_wait(&s_empty[sb], ((j / C::SB) & 1) ^ 1);
-          tc_fence_after();
-          astamp(1, j, 1);
-          uint8_t* sK = sKV + st_s * (C::K_BYTES + C::V_BYTES);
-#pragma unroll
-          for (int kk = 0; kk < C::KSTEPS; ++kk) {
-            uint64_t ad = make_desc_sw128(smem_u32(sQ + (kk >> 2) * 16384)) + 2 * (kk & 3);
-            uint64_t bd = make_desc_sw128(smem_u32(sK + (kk >> 2) * (C::BKV * 128))) + 2 * (kk & 3);
-            umma_bf16(tmem + sb * C::BKV, ad, bd, idesc_s, kk > 0 ? 1u : 0u);
-          }
-          umma_commit(&s_full[sb]);
-          if (++st_s == C::STAGES) {
-            st_s = 0;
-            ph_s ^= 1;
-          }
-        }
-        if (j >= 1) {
-          const int jj = j - 1, pb = jj % C::PB;
-          astamp(1, jj, 2);
-          mbar_wait(&p_full[pb], (jj / C::PB) & 1);     // P_jj in smem, O rescaled if the reference moved
-          tc_fence_after();
-          astamp(1, jj, 3);
-          uint8_t* sV = sKV + st_p * (C::K_BYTES + C::V_BYTES) + C::K_BYTES;
-          uint8_t* sPb = sP + pb * C::P_BYTES;
-          const int kv_valid = min(C::BKV, p.nk - jj * C::BKV);
-          const int ksteps = (kv_valid + 15) >> 4;
-          for (int kk = 0; kk < ksteps; ++kk) {
-            uint64_t ad = make_desc_sw128(smem_u32(sPb + (kk >> 2) * 16384)) + 2 * (kk & 3);
-            uint64_t bd = make_desc_sw128(smem_u32(sV + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
-            umma_bf16(tmem + C::O_COL0, ad, bd, idesc_o, (jj > 0 || kk > 0) ? 1u : 0u);   // O += P_jj V_jj
-          }
-          umma_commit(&o_full);
-          umma_commit(&p_empty[pb]);
-          umma_commit(&kv_empty[st_p]);
-          if (++st_p == C::STAGES) st_p = 0;
-        }
-      }
-      umma_commit(&o_done);   // every PV product has retired
-    }
-  } else {
-    // ================================================================= softmax (warps 0..3), one thread per query row
-    const int r = warp * 32 + lane;  // query row in tile == TMEM lane
-    const uint32_t trow = tmem + (uint32_t(warp * 32) << 16);
-    const int q_idx = q0 + r;
-    const float c = p.scale_log2;
-    float m = -INFINITY, l = 0.f, a_pend = 1.f;
-    const bool want_pc = p.pcols != nullptr;
-    int pos0 = -1, pos1 = -1;
-    if (want_pc) {
-      const int bb = bh / p.heads;
-      pos0 = __ldg(p.pos + bb * 2);
-      pos1 = __ldg(p.pos + bb * 2 + 1);
-    }
+    return;
+  }
 
-    for (int j = 0; j < T; ++j) {
-      const int sb = j % C::SB, pbuf = j % C::PB;
-      const int kv_valid = min(C::BKV, p.nk - j * C::BKV);
-      if (threadIdx.x == 0) astamp(0, j, 0);
-      if (lane == 0) mbar_wait(&s_full[sb], (j / C::SB) & 1);
-      __syncwarp();
-      tc_fence_after();
-      if (threadIdx.x == 0) astamp(0, j, 1);
-      const uint32_t ts = trow + sb * C::BKV;
-      const uint32_t sPb = smem_u32(sP + pbuf * C::P_BYTES);
-      const uint32_t pe_parity = ((j / C::PB) & 1) ^ 1;
-      // causal (CLIP text encoder, self-attention): row q attends to keys <= q
+  // =================================================================== consumers: rows rA, rA + 8 of the tile
+  const int wg = warp >> 2;
+  const int rA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const float c = p.scale_log2;
+  const bool want_pc = p.pcols != nullptr;
+  int pos0 = -1, pos1 = -1;
+  if (want_pc) {
+    const int bb = bh / p.heads;
+    pos0 = __ldg(p.pos + bb * 2);
+    pos1 = __ldg(p.pos + bb * 2 + 1);
+  }
+  float o[NO];
+#pragma unroll
+  for (int i = 0; i < NO; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, pc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+  mbar_wait(&q_full, 0);
+  const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + wg * (64 * 128)));
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < T; ++j) {
+    mbar_wait(&kv_full[st], ph);
+    uint8_t* sK = sKV + st * (C::K_BYTES + C::V_BYTES);
+    uint8_t* sV = sK + C::K_BYTES;
+    float s[NS];
+#pragma unroll
+    for (int i = 0; i < NS; ++i) s[i] = 0.f;
+    wgmma_fence_regs(s);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < C::KSTEPS; ++kk) {
+      const uint64_t kd = make_desc_sw128(smem_u32(sK + (kk >> 2) * (C::BKV * 128)));
+      wgmma_ss<C::BKV, F16>(s, qdesc + (kk >> 2) * (16384 >> 4) + 2 * (kk & 3), kd + 2 * (kk & 3), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // ---- online softmax (log2 domain); masked columns -> probability 0
+    const int kv_valid = min(C::BKV, p.nk - j * C::BKV);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int q_idx = q0 + rA + 8 * hr;
       const int row_lim = CAUSAL ? max(0, min(kv_valid, q_idx - j * C::BKV + 1)) : kv_valid;
-      float m_use = m;
-      if (j == 0) m_use = s_row_max<C::BKV>(ts, kv_valid, row_lim) * c;    // the only two-pass tile
-      float rs, mx, mt, pc0 = 0.f, pc1 = 0.f;
-      const bool fast = !CAUSAL && kv_valid == C::BKV && !want_pc;
-      if (fast) s_softmax_pass_full<C::BKV, F16>(ts, c, m_use, sPb, r, &p_empty[pbuf], pe_parity, lane, rs, mx);
-      else if (want_pc)
-        s_softmax_pass<C::BKV, true, F16>(ts, c, m_use, kv_valid, row_lim, sPb, r, &p_empty[pbuf], pe_parity, true, lane, rs, mx,
-                                     pos0 - j * C::BKV, pos1 - j * C::BKV, pc0, pc1);
-      else
-        s_softmax_pass<C::BKV, false, F16>(ts, c, m_use, kv_valid, row_lim, sPb, r, &p_empty[pbuf], pe_parity, true, lane, rs, mx, -1,
-                                      -1, pc0, pc1);
-      mt = mx * c;
-      if (j > 0 && __any_sync(0xffffffffu, mt > m_use + 32.f)) {
-        // slow path: a logit far above everything seen so far -- redo this tile against its own maximum
-        const float m_new = fmaxf(m_use, mt);
-        const float a = ex2_approx(m - m_new);
-        l *= a;
-        a_pend *= a;
-        m_use = m_new;
-        if (want_pc)
-          s_softmax_pass<C::BKV, true, F16>(ts, c, m_use, kv_valid, row_lim, sPb, r, &p_empty[pbuf], pe_parity, false, lane, rs, mx,
-                                       pos0 - j * C::BKV, pos1 - j * C::BKV, pc0, pc1);
-        else
-          s_softmax_pass<C::BKV, false, F16>(ts, c, m_use, kv_valid, row_lim, sPb, r, &p_empty[pbuf], pe_parity, false, lane, rs,
-                                        mx, -1, -1, pc0, pc1);
-        mt = mx * c;
-      }
-      l += rs;
-      m = m_use;
-      if (threadIdx.x == 0) astamp(0, j, 2);
-      if (j > 0 && __any_sync(0xffffffffu, a_pend != 1.f)) {
-        // the reference moved: rescale this row of O (tiles < j) in TMEM before PV_j may accumulate onto it
-        if (lane == 0) mbar_wait(&o_full, (j - 1) & 1);
-        __syncwarp();
-        tc_fence_after();
+      float mx = -INFINITY;
 #pragma unroll
-        for (int cc = 0; cc < C::DV / 16; ++cc) {
-          uint32_t v[16];
-          tmem_ld16(trow + C::O_COL0 + cc * 16, v);
-          tmem_ld_wait();
+      for (int i = 0; i < C::BKV / 8; ++i)
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * a_pend);
-          tmem_st16(trow + C::O_COL0 + cc * 16, v);
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * i + cq + e;
+          float& x = s[4 * i + 2 * hr + e];
+          x = col < row_lim ? x * c : -INFINITY;
+          mx = fmaxf(mx, x);
         }
-        tmem_st_wait();
-        a_pend = 1.f;
-      }
-      if (want_pc && T == 1 && q_idx < p.nq) {
-        const float inv = 1.0f / rs;
-        *reinterpret_cast<float2*>(p.pcols + ((long long)bh * p.nq + q_idx) * 2) = make_float2(pc0 * inv, pc1 * inv);
-      }
-      if (p.probs != nullptr && T == 1) {
-        // normalised probabilities for the attention controller (edlora.py:81-82): single kv tile, so l = rs
-        const float inv = 1.0f / rs;
-        float* prow = p.probs + ((long long)bh * p.nq + q_idx) * p.nk;
-#pragma unroll 1
-        for (int cc = 0; cc < C::BKV / 32; ++cc) {
-          uint32_t v[32];
-          tmem_ld32(ts + cc * 32, v);
-          tmem_ld_wait();
-          if (q_idx < p.nq) {
+      mx = quad_max(mx);
+      const float m_new = fmaxf(m[hr], mx);
+      const float m_use = m_new == -INFINITY ? 0.f : m_new;   // fully masked so far: keep everything at 0
+      const float alpha = ex2_approx(m[hr] - m_use);
+      m[hr] = m_new;
+      l[hr] *= alpha;
+      pc[hr][0] *= alpha;
+      pc[hr][1] *= alpha;
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (cc * 32 + i < kv_valid) prow[cc * 32 + i] = exp2f(__uint_as_float(v[i]) * c - m_use) * inv;
+      for (int i = 0; i < C::DV / 8; ++i) {
+        o[4 * i + 2 * hr] *= alpha;
+        o[4 * i + 2 * hr + 1] *= alpha;
+      }
+      float rs = 0.f;
+#pragma unroll
+      for (int i = 0; i < C::BKV / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& x = s[4 * i + 2 * hr + e];
+          x = ex2_approx(x - m_use);
+          rs += x;
+          if (want_pc) {
+            const int kcol = j * C::BKV + 8 * i + cq + e;
+            if (kcol == pos0) pc[hr][0] += x;
+            if (kcol == pos1) pc[hr][1] += x;
           }
-          __syncwarp();
         }
-      }
-      tc_fence_before();              // this thread's TMEM reads of S_j (and O rescale) are ordered before ...
-      fence_proxy_async_smem();       // ... and its P_j stores are visible to the tensor core's async proxy
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&s_empty[sb]);
-        mbar_arrive(&p_full[pbuf]);
-      }
-      if (threadIdx.x == 0) astamp(0, j, 3);
-      // lazy reference update for the following tiles (applied to O -- including PV_j -- before P_{j+1} is published)
-      if (mt > m + 8.f) {
-        const float a = ex2_approx(m - mt);
-        l *= a;
-        a_pend *= a;
-        m = mt;
+      l[hr] += rs;
+    }
+    if (p.probs != nullptr && T == 1) {
+      // normalised probabilities for the attention controller (edlora.py:81-82): single kv tile
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int q_idx = q0 + rA + 8 * hr;
+        const float inv = 1.0f / quad_sum(l[hr]);
+        if (q_idx < p.nq) {
+          float* prow = p.probs + ((long long)bh * p.nq + q_idx) * p.nk;
+#pragma unroll
+          for (int i = 0; i < C::BKV / 8; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (8 * i + cq + e < kv_valid) prow[8 * i + cq + e] = s[4 * i + 2 * hr + e] * inv;
+        }
       }
     }
-    // all PV products retired -> normalise and write the row
-    // (o_full cannot be used here: with two P buffers PV_{T-2} may still be in flight, and a parity wait cannot tell
-    // "T - 2 completions" from "T completions")
-    if (lane == 0) mbar_wait(&o_done, 0);
+    // ---- O += P V (P from registers; k-steps past the last valid key are skipped: those columns of V^T may be padding)
+    const int ksteps = (kv_valid + 15) >> 4;
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < C::BKV / 16; ++kk) {
+      if (kk < ksteps) {
+        uint32_t a[4];
+        frag_to_a<F16>(&s[8 * kk], a);
+        const uint64_t vd = make_desc_sw128(smem_u32(sV + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
+        wgmma_rs<C::DV, F16>(o, a, vd, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
     __syncwarp();
-    tc_fence_after();
-    const float inv = a_pend / l;
-    const int b = bh / p.heads, h = bh - b * p.heads;
-    if (q_idx < p.nq && p.lse2 != nullptr) p.lse2[(long long)bh * p.nq + q_idx] = m + log2f(l);
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+    if (++st == C::STAGES) {
+      st = 0;
+      ph ^= 1;
+    }
+  }
+  // ---- normalise and write the two rows
+  const int b = bh / p.heads, h = bh - b * p.heads;
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q_idx = q0 + rA + 8 * hr;
+    const float lt = quad_sum(l[hr]);
+    const float inv = 1.0f / lt;
+    if (want_pc && T == 1) {
+      const float p0 = quad_sum(pc[hr][0]), p1 = quad_sum(pc[hr][1]);
+      if (q_idx < p.nq && (lane & 3) == 0)
+        *reinterpret_cast<float2*>(p.pcols + ((long long)bh * p.nq + q_idx) * 2) = make_float2(p0 * inv, p1 * inv);
+    }
+    if (q_idx >= p.nq) continue;
+    if (p.lse2 != nullptr && (lane & 3) == 0) p.lse2[(long long)bh * p.nq + q_idx] = m[hr] + log2f(lt);
     __nv_bfloat16* orow = p.out + ((long long)b * p.nq + q_idx) * p.ldo + h * D;
 #pragma unroll
-    for (int cc = 0; cc < C::DV / 16; ++cc) {
-      uint32_t v[16];
-      tmem_ld16(trow + C::O_COL0 + cc * 16, v);
-      tmem_ld_wait();
-      if (q_idx < p.nq) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (cc * 16 + g * 8 < D) {
-            uint4 u;
-            u.x = pack16x2<F16>(__uint_as_float(v[g * 8 + 0]) * inv, __uint_as_float(v[g * 8 + 1]) * inv);
-            u.y = pack16x2<F16>(__uint_as_float(v[g * 8 + 2]) * inv, __uint_as_float(v[g * 8 + 3]) * inv);
-            u.z = pack16x2<F16>(__uint_as_float(v[g * 8 + 4]) * inv, __uint_as_float(v[g * 8 + 5]) * inv);
-            u.w = pack16x2<F16>(__uint_as_float(v[g * 8 + 6]) * inv, __uint_as_float(v[g * 8 + 7]) * inv);
-            *reinterpret_cast<uint4*>(orow + cc * 16 + g * 8) = u;
-          }
-        }
-      }
+    for (int i = 0; i < C::DV / 8; ++i) {
+      const int col = 8 * i + cq;
+      if (col < D)
+        *reinterpret_cast<uint32_t*>(orow + col) = pack16x2<F16>(o[4 * i + 2 * hr] * inv, o[4 * i + 2 * hr + 1] * inv);
     }
-    tc_fence_before();
-  }
-
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::TMEM_COLS);
   }
 }
-
-static unsigned long long* g_attn_tl_host = nullptr;
 
 template <int D, bool ONE, bool CAUSAL = false, bool F16 = false>
 static int launch_attn(const void* Q, const void* K, const void* Vt, void* out, int64_t ldo, float* probs, int BH,
@@ -531,19 +310,13 @@ static int launch_attn(const void* Q, const void* K, const void* Vt, void* out, 
   p.lse2 = lse2;
   p.pcols = pcols;
   p.pos = pos;
-  p.tl = g_attn_tl_host;
   static bool configured = false;
   if (!configured) {
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<D, ONE, false, CAUSAL, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    if (!CAUSAL && !F16)
-      MOS_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<D, ONE, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<D, ONE, CAUSAL, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
   dim3 grid((unsigned)ceil_div(nq, 128), (unsigned)BH);
-  if (!CAUSAL && !F16 && p.tl != nullptr)
-    MOS_CHECK_CUDA(launch_pdl(attn_kernel<D, ONE, true, false, false>, grid, dim3(192), (size_t)C::SMEM_BYTES, stream, tmQ, tmK, tmV, p));
-  else
-    MOS_CHECK_CUDA(launch_pdl(attn_kernel<D, ONE, false, CAUSAL, F16>, grid, dim3(192), (size_t)C::SMEM_BYTES, stream, tmQ, tmK, tmV, p));
+  MOS_CHECK_CUDA(launch_pdl(attn_kernel<D, ONE, CAUSAL, F16>, grid, dim3(ATTN_THREADS), (size_t)C::SMEM_BYTES, stream, tmQ, tmK, tmV, p));
   return MOS_OK;
 }
 
@@ -619,9 +392,4 @@ extern "C" int mos_attention_fwd_causal(const void* Q, const void* K, const void
   MOS_CHECK_ARG(ldo >= (int64_t)heads * head_dim && ldo % 8 == 0, "mos_attention_fwd_causal: bad ldo");
   if (head_dim != 80) return set_err(MOS_EUNSUPPORTED, "mos_attention_fwd_causal: head_dim %d (only 80 is built)", head_dim);
   return launch_attn<80, true, true>(Q, K, Vt, out, ldo, nullptr, batch * heads, heads, n, n, n8, scale, stream, lse2);
-}
-
-extern "C" int mos_debug_set_attn_timeline(void* buf) {
-  mos::g_attn_tl_host = reinterpret_cast<unsigned long long*>(buf);
-  return MOS_OK;
 }

@@ -1,5 +1,5 @@
-// attention_bwd.cu — flash-attention backward on tcgen05 for d = 40 / 80 / 160 (training step, trainer_edlora.py:237
-// reached through loss.backward(); forward counterpart: attention.cu).
+// attention_bwd.cu — flash-attention backward on wgmma (sm_90a) for d = 40 / 80 / 160 (training step,
+// trainer_edlora.py:237 reached through loss.backward(); forward counterpart: attention.cu).
 //
 //   P = softmax(S), S = scale Q K^T ;  O = P V ;  given dO:
 //   dV = P^T dO ;  dP = dO V^T ;  dS = P o (dP + G - delta) ;  dQ = scale dS K ;  dK = scale dS^T Q
@@ -7,12 +7,13 @@
 //   regulariser, trainer_edlora.py:263-313: two key columns per sample, identical over heads).
 //
 // Two kernels, both recompute P from the saved log-sum-exp (no atomics, no N x N tensor in HBM):
-//   attn_bwd_dq_kernel   one CTA per 128-query tile, loops over key tiles:  S, dP on the tensor cores -> dS (bf16,
-//                        swizzled smem) -> dQ += dS K accumulated in TMEM
-//   attn_bwd_dkv_kernel  one CTA per 128-key tile, loops over query tiles: S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T ->
-//                        dV += P^T dO, dK += dS^T Q accumulated in TMEM
-// Warp roles as in the forward kernel: warps 0..3 own one TMEM lane (row) each, warp 4 = TMA producer, warp 5 = MMA.
-// Operand layouts: rows [B*H, R, DP] and transposed [B*H, DV, R8] copies (mos_heads_transpose) so that every MMA
+//   attn_bwd_dq_kernel   one CTA per 128-query tile, loops over key tiles:  S, dP (wgmma, registers) -> dS in registers
+//                        -> dQ += dS K (wgmma with dS as the register A operand)
+//   attn_bwd_dkv_kernel  one CTA per 128-key tile, loops over query tiles: S^T = K Q^T, dP^T = V dO^T -> P^T, dS^T in
+//                        registers -> dV += P^T dO, dK += dS^T Q.  For d = 160 the dK / dV columns are split over two CTAs
+//                        (gridDim.z) so that both accumulators fit the register file.
+// Roles as in the forward kernel: two consumer warpgroups of 64 rows each, warp 8 = TMA producer.
+// Operand layouts: rows [B*H, R, DP] and transposed [B*H, DV, R8] copies (mos_heads_transpose) so that every shared-memory
 // operand is K-major SWIZZLE_128B.  Outputs are token-major [B*R, ld] bf16 (head h in columns h*d ..).
 #include "common.h"
 #include "tc.cuh"
@@ -31,35 +32,26 @@ struct BwdCfg {
   static constexpr int DP = ((D + 63) / 64) * 64;
   static constexpr int QCH = DP / 64;
   static constexpr int DV = ((D + 15) / 16) * 16;
-  static constexpr int OSTR = ((DV + 63) / 64) * 64;
-  // ---- dQ kernel: inner tile = keys
-  // d = 40: 64-wide inner tiles, 256 TMEM columns and <= 113 KB smem, so that TWO CTAs share an SM: every tile is a
-  // serial chain (S, dP on the tensor pipe -> dS by the row threads -> dQ), and the second CTA fills the bubbles.
-  static constexpr int BTA = D <= 40 ? 64 : (D <= 80 ? 128 : 64);
-  static constexpr int MINB = D <= 40 ? 2 : 1;
-  static constexpr int KCHA = BTA / 64;
+  static constexpr int BT = 64;                               // inner tile (keys for dQ, queries for dK / dV)
+  static constexpr int STAGES = D <= 80 ? 2 : 1;
+  // ---- dQ kernel
   static constexpr int A_Q_BYTES = QCH * 128 * 128;           // Q or dO tile [128, DP]
-  static constexpr int A_K_BYTES = QCH * BTA * 128;           // K or V tile [BTA, DP]
-  static constexpr int A_KT_BYTES = KCHA * DV * 128;          // K^T tile [DV, BTA]
-  static constexpr int A_DS_BYTES = KCHA * 128 * 128;         // dS [128, BTA]
-  static constexpr int A_SMEM = 2 * A_Q_BYTES + 2 * A_K_BYTES + A_KT_BYTES + A_DS_BYTES + 1024;
-  static constexpr int A_DQ_COL = 2 * BTA;
-  static constexpr int A_TMEM = (A_DQ_COL + OSTR <= 256) ? 256 : 512;
-  static_assert(A_DQ_COL + OSTR <= A_TMEM, "TMEM budget (dq)");
-  // ---- dK/dV kernel: inner tile = queries
-  static constexpr int BTB = 64;
-  static constexpr int KCHB = BTB / 64;
+  static constexpr int A_K_BYTES = QCH * BT * 128;            // K or V tile [BT, DP]
+  static constexpr int A_KT_BYTES = DV * 128;                 // K^T tile [DV, BT]
+  static constexpr int A_STAGE = 2 * A_K_BYTES + A_KT_BYTES;
+  static constexpr int A_SMEM = 2 * A_Q_BYTES + STAGES * A_STAGE + 1024;
+  // ---- dK/dV kernel
+  static constexpr int DVH = D <= 80 ? DV : DV / 2;           // output columns per CTA
+  static constexpr int ZSPLIT = DV / DVH;
   static constexpr int B_K_BYTES = QCH * 128 * 128;           // K or V tile [128, DP]
-  static constexpr int B_Q_BYTES = QCH * BTB * 128;           // Q or dO tile [BTB, DP]
-  static constexpr int B_QT_BYTES = KCHB * DV * 128;          // Q^T or dO^T tile [DV, BTB]
-  static constexpr int B_P_BYTES = KCHB * 128 * 128;          // P^T or dS^T [128, BTB]
-  static constexpr int B_SMEM = 2 * B_K_BYTES + 2 * B_Q_BYTES + 2 * B_QT_BYTES + 2 * B_P_BYTES + 1024;
-  static constexpr int B_DK_COL = 2 * BTB;
-  static constexpr int B_DV_COL = 2 * BTB + OSTR;
-  static constexpr int B_TMEM = (B_DV_COL + OSTR <= 256) ? 256 : 512;
-  static_assert(B_DV_COL + OSTR <= B_TMEM, "TMEM budget (dkv)");
+  static constexpr int B_Q_BYTES = QCH * BT * 128;            // Q or dO tile [BT, DP]
+  static constexpr int B_QT_BYTES = DV * 128;                 // Q^T or dO^T tile [DV, BT]
+  static constexpr int B_STAGE = 2 * B_Q_BYTES + 2 * B_QT_BYTES;
+  static constexpr int B_SMEM = 2 * B_K_BYTES + STAGES * B_STAGE + 1024;
   static_assert(A_SMEM <= 227 * 1024 - 2048 && B_SMEM <= 227 * 1024 - 2048, "smem budget");
 };
+
+constexpr int BWD_THREADS = 256 + 32;
 
 struct BwdDev {
   int nq, nk, heads;
@@ -77,73 +69,56 @@ struct BwdDev {
   long long lddv;
 };
 
-// write 32 consecutive fp32 values of row r as bf16 into a [128 x 64-col chunks] SWIZZLE_128B K-major tile
-__device__ __forceinline__ void store_row32_sw128(uint8_t* tile, int r, int c /* 32-col chunk index */, const float* v) {
-  uint8_t* rowp = tile + (c >> 1) * 16384 + r * 128;
+// S = A_rows B_rows^T over the head dimension: KSTEPS k16 steps over 64-column chunks of [rows, DP] tiles
+template <int D, int ROWS_B>
+__device__ __forceinline__ void bwd_rows_product(float (&s)[BwdCfg<D>::BT / 2], const uint8_t* sa, const uint8_t* sb) {
+  using C = BwdCfg<D>;
+  const uint64_t ad = make_desc_sw128(smem_u32(sa)), bd = make_desc_sw128(smem_u32(sb));
 #pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    uint4 u;
-    u.x = pack_bf16x2(v[g * 8 + 0], v[g * 8 + 1]);
-    u.y = pack_bf16x2(v[g * 8 + 2], v[g * 8 + 3]);
-    u.z = pack_bf16x2(v[g * 8 + 4], v[g * 8 + 5]);
-    u.w = pack_bf16x2(v[g * 8 + 6], v[g * 8 + 7]);
-    const int c16 = (c & 1) * 4 + g;
-    *reinterpret_cast<uint4*>(rowp + ((c16 ^ (r & 7)) << 4)) = u;
-  }
+  for (int kk = 0; kk < C::KSTEPS; ++kk)
+    wgmma_ss<C::BT, false>(s, ad + (kk >> 2) * (16384 >> 4) + 2 * (kk & 3),
+                           bd + (kk >> 2) * ((ROWS_B * 128) >> 4) + 2 * (kk & 3), 1u);
 }
 
 // =================================================================================================== dQ
 template <int D>
-__global__ void __launch_bounds__(192, BwdCfg<D>::MINB)
+__global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                    const __grid_constant__ CUtensorMap tmKt, const BwdDev p) {
   using C = BwdCfg<D>;
-  constexpr int BT = C::BTA;
+  constexpr int BT = C::BT, NS = BT / 2, NO = C::DV / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sdO = sQ + C::A_Q_BYTES;
-  uint8_t* sK = sdO + C::A_Q_BYTES;
-  uint8_t* sV = sK + C::A_K_BYTES;
-  uint8_t* sKt = sV + C::A_K_BYTES;
-  uint8_t* sdS = sKt + C::A_KT_BYTES;
+  uint8_t* sStages = sdO + C::A_Q_BYTES;
 
-  __shared__ uint64_t qdo_full, kv_full, kv_empty, kt_full, kt_empty, sdp_full, sdp_empty, ds_full, ds_empty, dq_full;
-  __shared__ uint32_t tmem_holder;
+  __shared__ uint64_t qdo_full, kv_full[C::STAGES], kv_empty[C::STAGES];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
   const int T = (p.nk + BT - 1) / BT;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmdO);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmKt);
     mbar_init(&qdo_full, 1);
-    mbar_init(&kv_full, 1);
-    mbar_init(&kv_empty, 1);
-    mbar_init(&kt_full, 1);
-    mbar_init(&kt_empty, 1);
-    mbar_init(&sdp_full, 1);
-    mbar_init(&sdp_empty, 128);
-    mbar_init(&ds_full, 128);
-    mbar_init(&ds_empty, 1);
-    mbar_init(&dq_full, 1);
+    for (int s = 0; s < C::STAGES; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 8);
+    }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(&tmem_holder, C::A_TMEM);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_holder;
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(&qdo_full, 2 * C::A_Q_BYTES);
 #pragma unroll
@@ -151,172 +126,148 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         tma_load_3d(sQ + c * 16384, &tmQ, &qdo_full, c * 64, q0, bh);
         tma_load_3d(sdO + c * 16384, &tmdO, &qdo_full, c * 64, q0, bh);
       }
-      // K / V row tiles are only read by the S and dP products and K^T only by the dQ product: each buffer is released
-      // as soon as its last reader has retired, so the next tile's loads fly while the row threads compute dS.
+      int st = 0;
+      uint32_t ph = 0;
       for (int j = 0; j < T; ++j) {
-        mbar_wait(&kv_empty, (j & 1) ^ 1);
-        mbar_expect_tx(&kv_full, 2 * C::A_K_BYTES);
+        uint8_t* sK = sStages + st * C::A_STAGE;
+        uint8_t* sV = sK + C::A_K_BYTES;
+        uint8_t* sKt = sV + C::A_K_BYTES;
+        mbar_wait_hint(&kv_empty[st], ph ^ 1);
+        mbar_expect_tx(&kv_full[st], C::A_STAGE);
 #pragma unroll
         for (int c = 0; c < C::QCH; ++c) {
-          tma_load_3d(sK + c * (BT * 128), &tmK, &kv_full, c * 64, j * BT, bh);
-          tma_load_3d(sV + c * (BT * 128), &tmV, &kv_full, c * 64, j * BT, bh);
+          tma_load_3d(sK + c * (BT * 128), &tmK, &kv_full[st], c * 64, j * BT, bh);
+          tma_load_3d(sV + c * (BT * 128), &tmV, &kv_full[st], c * 64, j * BT, bh);
         }
-        mbar_wait(&kt_empty, (j & 1) ^ 1);
-        mbar_expect_tx(&kt_full, C::A_KT_BYTES);
-#pragma unroll
-        for (int c = 0; c < C::KCHA; ++c)
-          tma_load_3d(sKt + c * (C::DV * 128), &tmKt, &kt_full, j * BT + c * 64, 0, bh);
-      }
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc(128, BT, 1);
-      const uint32_t idesc_o = make_idesc(128, C::DV, 1);
-      mbar_wait(&qdo_full, 0);
-      for (int j = 0; j < T; ++j) {
-        mbar_wait(&kv_full, j & 1);
-        mbar_wait(&sdp_empty, (j & 1) ^ 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < C::KSTEPS; ++kk) {
-          const uint64_t aq = make_desc_sw128(smem_u32(sQ + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bk = make_desc_sw128(smem_u32(sK + (kk >> 2) * (BT * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem, aq, bk, idesc_s, kk > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < C::KSTEPS; ++kk) {
-          const uint64_t ad = make_desc_sw128(smem_u32(sdO + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bv = make_desc_sw128(smem_u32(sV + (kk >> 2) * (BT * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem + BT, ad, bv, idesc_s, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&sdp_full);
-        umma_commit(&kv_empty);          // K / V row tiles are free once S and dP have retired
-        mbar_wait(&ds_full, j & 1);
-        mbar_wait(&kt_full, j & 1);
-        tc_fence_after();
-        const int kv_valid = min(BT, p.nk - j * BT);
-        const int ksteps = (kv_valid + 15) >> 4;
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint64_t as = make_desc_sw128(smem_u32(sdS + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bt = make_desc_sw128(smem_u32(sKt + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem + C::A_DQ_COL, as, bt, idesc_o, (j > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&ds_empty);
-        umma_commit(&kt_empty);
-      }
-      umma_commit(&dq_full);
-    }
-  } else {
-    const int r = warp * 32 + lane;
-    const uint32_t trow = tmem + (uint32_t(warp * 32) << 16);
-    const int q_idx = q0 + r;
-    const bool row_ok = q_idx < p.nq;
-    const int b = bh / p.heads, h = bh - b * p.heads;
-    const float lse = row_ok ? __ldg(p.lse2 + (long long)bh * p.nq + q_idx) : INFINITY;
-    const float dl = row_ok ? __ldg(p.delta + (long long)bh * p.nq + q_idx) : 0.f;
-    float g0 = 0.f, g1 = 0.f;
-    int pos0 = -1, pos1 = -1;
-    if (p.gcols != nullptr) {
-      pos0 = __ldg(p.pos + b * 2);
-      pos1 = __ldg(p.pos + b * 2 + 1);
-      if (row_ok) {
-        g0 = __ldg(p.gcols + ((long long)b * p.nq + q_idx) * 2);
-        g1 = __ldg(p.gcols + ((long long)b * p.nq + q_idx) * 2 + 1);
-      }
-    }
-    for (int j = 0; j < T; ++j) {
-      const int kv_valid = min(BT, p.nk - j * BT);
-      if (lane == 0) {
-        mbar_wait(&sdp_full, j & 1);
-        if (j > 0) mbar_wait(&ds_empty, (j - 1) & 1);
-      }
-      __syncwarp();
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BT / 32; ++c) {
-        uint32_t sv[32], dv[32];
-        tmem_ld32(trow + c * 32, sv);
-        tmem_ld32(trow + BT + c * 32, dv);
-        tmem_ld_wait();
-        float ds[32];
-        const int k0 = j * BT + c * 32;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float pr = ex2_approx_b(fmaf(__uint_as_float(sv[i]), p.scale_log2, -lse));
-          pr = (c * 32 + i < kv_valid && (!p.causal || k0 + i <= q_idx)) ? pr : 0.f;
-          float dp = __uint_as_float(dv[i]);
-          if (p.gcols != nullptr) dp += (k0 + i == pos0) ? g0 : ((k0 + i == pos1) ? g1 : 0.f);
-          ds[i] = pr * (dp - dl) * p.scale;
-        }
-        store_row32_sw128(sdS, r, c, ds);
-      }
-      tc_fence_before();
-      mbar_arrive(&sdp_empty);
-      fence_proxy_async_smem();
-      mbar_arrive(&ds_full);
-    }
-    if (lane == 0) mbar_wait(&dq_full, 0);
-    __syncwarp();
-    tc_fence_after();
-    __nv_bfloat16* orow = p.dq + ((long long)b * p.nq + q_idx) * p.lddq + h * D;
-#pragma unroll 1
-    for (int c = 0; c < C::DV / 16; ++c) {
-      uint32_t v[16];
-      tmem_ld16(trow + C::A_DQ_COL + c * 16, v);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c * 16 + g * 8 < D) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v[g * 8 + 0]), __uint_as_float(v[g * 8 + 1]));
-            u.y = pack_bf16x2(__uint_as_float(v[g * 8 + 2]), __uint_as_float(v[g * 8 + 3]));
-            u.z = pack_bf16x2(__uint_as_float(v[g * 8 + 4]), __uint_as_float(v[g * 8 + 5]));
-            u.w = pack_bf16x2(__uint_as_float(v[g * 8 + 6]), __uint_as_float(v[g * 8 + 7]));
-            *reinterpret_cast<uint4*>(orow + c * 16 + g * 8) = u;
-          }
+        tma_load_3d(sKt, &tmKt, &kv_full[st], j * BT, 0, bh);
+        if (++st == C::STAGES) {
+          st = 0;
+          ph ^= 1;
         }
       }
     }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::A_TMEM);
+
+  const int wg = warp >> 2;
+  const int rA = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const int b = bh / p.heads, h = bh - b * p.heads;
+  float lse[2], dl[2], g0[2] = {0.f, 0.f}, g1[2] = {0.f, 0.f};
+  int pos0 = -1, pos1 = -1;
+  if (p.gcols != nullptr) {
+    pos0 = __ldg(p.pos + b * 2);
+    pos1 = __ldg(p.pos + b * 2 + 1);
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q_idx = q0 + rA + 8 * hr;
+    const bool row_ok = q_idx < p.nq;
+    lse[hr] = row_ok ? __ldg(p.lse2 + (long long)bh * p.nq + q_idx) : INFINITY;
+    dl[hr] = row_ok ? __ldg(p.delta + (long long)bh * p.nq + q_idx) : 0.f;
+    if (p.gcols != nullptr && row_ok) {
+      g0[hr] = __ldg(p.gcols + ((long long)b * p.nq + q_idx) * 2);
+      g1[hr] = __ldg(p.gcols + ((long long)b * p.nq + q_idx) * 2 + 1);
+    }
+  }
+  float dq[NO];
+#pragma unroll
+  for (int i = 0; i < NO; ++i) dq[i] = 0.f;
+  mbar_wait(&qdo_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < T; ++j) {
+    uint8_t* sK = sStages + st * C::A_STAGE;
+    uint8_t* sV = sK + C::A_K_BYTES;
+    uint8_t* sKt = sV + C::A_K_BYTES;
+    mbar_wait(&kv_full[st], ph);
+    float s[NS], dp[NS];
+#pragma unroll
+    for (int i = 0; i < NS; ++i) s[i] = dp[i] = 0.f;
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    wgmma_fence();
+    bwd_rows_product<D, BT>(s, sQ + wg * (64 * 128), sK);
+    bwd_rows_product<D, BT>(dp, sdO + wg * (64 * 128), sV);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    const int kv_valid = min(BT, p.nk - j * BT);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int q_idx = q0 + rA + 8 * hr;
+#pragma unroll
+      for (int i = 0; i < BT / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * i + cq + e, key = j * BT + col;
+          const int x = 4 * i + 2 * hr + e;
+          float pr = ex2_approx_b(fmaf(s[x], p.scale_log2, -lse[hr]));
+          pr = (col < kv_valid && (!p.causal || key <= q_idx)) ? pr : 0.f;
+          float d = dp[x];
+          if (p.gcols != nullptr) d += (key == pos0) ? g0[hr] : ((key == pos1) ? g1[hr] : 0.f);
+          s[x] = pr * (d - dl[hr]) * p.scale;     // dS
+        }
+    }
+    const int ksteps = (kv_valid + 15) >> 4;
+    wgmma_fence_regs(dq);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BT / 16; ++kk) {
+      if (kk < ksteps) {
+        uint32_t a[4];
+        frag_to_a<false>(&s[8 * kk], a);
+        wgmma_rs<C::DV, false>(dq, a, make_desc_sw128(smem_u32(sKt)) + 2 * kk, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dq);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+    if (++st == C::STAGES) {
+      st = 0;
+      ph ^= 1;
+    }
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q_idx = q0 + rA + 8 * hr;
+    if (q_idx >= p.nq) continue;
+    __nv_bfloat16* orow = p.dq + ((long long)b * p.nq + q_idx) * p.lddq + h * D;
+#pragma unroll
+    for (int i = 0; i < C::DV / 8; ++i) {
+      const int col = 8 * i + cq;
+      if (col < D) *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16x2(dq[4 * i + 2 * hr], dq[4 * i + 2 * hr + 1]);
+    }
   }
 }
 
 // =================================================================================================== dK, dV
 template <int D>
-__global__ void __launch_bounds__(192, BwdCfg<D>::MINB)
+__global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                     const __grid_constant__ CUtensorMap tmQt, const __grid_constant__ CUtensorMap tmdOt,
                     const BwdDev p) {
   using C = BwdCfg<D>;
-  constexpr int BT = C::BTB;
+  constexpr int BT = C::BT, NS = BT / 2, NO = C::DVH / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = smem;
   uint8_t* sV = sK + C::B_K_BYTES;
-  uint8_t* sQ = sV + C::B_K_BYTES;
-  uint8_t* sdO = sQ + C::B_Q_BYTES;
-  uint8_t* sQt = sdO + C::B_Q_BYTES;
-  uint8_t* sdOt = sQt + C::B_QT_BYTES;
-  uint8_t* sPt = sdOt + C::B_QT_BYTES;
-  uint8_t* sdSt = sPt + C::B_P_BYTES;
+  uint8_t* sStages = sV + C::B_K_BYTES;
 
-  __shared__ uint64_t kv_full, q_full, q_empty, qt_full, qt_empty, stp_full, stp_empty, pds_full, pds_empty, out_full;
-  __shared__ uint32_t tmem_holder;
-  __shared__ float sL[2][BT], sDl[2][BT], sG0[2][BT], sG1[2][BT];
+  __shared__ uint64_t kv_full, q_full[C::STAGES], q_empty[C::STAGES];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
+  const int z = blockIdx.z;                  // output column block [z * DVH, z * DVH + DVH)
   const int T = (p.nq + BT - 1) / BT;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmQ);
@@ -324,26 +275,17 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     tma_prefetch_desc(&tmQt);
     tma_prefetch_desc(&tmdOt);
     mbar_init(&kv_full, 1);
-    mbar_init(&q_full, 1);
-    mbar_init(&q_empty, 1);
-    mbar_init(&qt_full, 1);
-    mbar_init(&qt_empty, 1);
-    mbar_init(&stp_full, 1);
-    mbar_init(&stp_empty, 128);
-    mbar_init(&pds_full, 128);
-    mbar_init(&pds_empty, 1);
-    mbar_init(&out_full, 1);
+    for (int s = 0; s < C::STAGES; ++s) {
+      mbar_init(&q_full[s], 1);
+      mbar_init(&q_empty[s], 8);
+    }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(&tmem_holder, C::B_TMEM);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_holder;
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(&kv_full, 2 * C::B_K_BYTES);
 #pragma unroll
@@ -351,161 +293,135 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         tma_load_3d(sK + c * 16384, &tmK, &kv_full, c * 64, k0, bh);
         tma_load_3d(sV + c * 16384, &tmV, &kv_full, c * 64, k0, bh);
       }
-      // Q / dO row tiles are only read by the S^T and dP^T products, Q^T / dO^T only by the dK / dV products: early
-      // release as in the dQ kernel.
+      int st = 0;
+      uint32_t ph = 0;
       for (int i = 0; i < T; ++i) {
-        mbar_wait(&q_empty, (i & 1) ^ 1);
-        mbar_expect_tx(&q_full, 2 * C::B_Q_BYTES);
+        uint8_t* sQ = sStages + st * C::B_STAGE;
+        uint8_t* sdO = sQ + C::B_Q_BYTES;
+        uint8_t* sQt = sdO + C::B_Q_BYTES;
+        uint8_t* sdOt = sQt + C::B_QT_BYTES;
+        mbar_wait_hint(&q_empty[st], ph ^ 1);
+        mbar_expect_tx(&q_full[st], C::B_STAGE);
 #pragma unroll
         for (int c = 0; c < C::QCH; ++c) {
-          tma_load_3d(sQ + c * (BT * 128), &tmQ, &q_full, c * 64, i * BT, bh);
-          tma_load_3d(sdO + c * (BT * 128), &tmdO, &q_full, c * 64, i * BT, bh);
+          tma_load_3d(sQ + c * (BT * 128), &tmQ, &q_full[st], c * 64, i * BT, bh);
+          tma_load_3d(sdO + c * (BT * 128), &tmdO, &q_full[st], c * 64, i * BT, bh);
         }
-        mbar_wait(&qt_empty, (i & 1) ^ 1);
-        mbar_expect_tx(&qt_full, 2 * C::B_QT_BYTES);
-#pragma unroll
-        for (int c = 0; c < C::KCHB; ++c) {
-          tma_load_3d(sQt + c * (C::DV * 128), &tmQt, &qt_full, i * BT + c * 64, 0, bh);
-          tma_load_3d(sdOt + c * (C::DV * 128), &tmdOt, &qt_full, i * BT + c * 64, 0, bh);
-        }
-      }
-    }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc(128, BT, 1);
-      const uint32_t idesc_o = make_idesc(128, C::DV, 1);
-      mbar_wait(&kv_full, 0);
-      for (int i = 0; i < T; ++i) {
-        mbar_wait(&q_full, i & 1);
-        mbar_wait(&stp_empty, (i & 1) ^ 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < C::KSTEPS; ++kk) {
-          const uint64_t ak = make_desc_sw128(smem_u32(sK + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bq = make_desc_sw128(smem_u32(sQ + (kk >> 2) * (BT * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem, ak, bq, idesc_s, kk > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < C::KSTEPS; ++kk) {
-          const uint64_t av = make_desc_sw128(smem_u32(sV + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bd = make_desc_sw128(smem_u32(sdO + (kk >> 2) * (BT * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem + BT, av, bd, idesc_s, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(&stp_full);
-        umma_commit(&q_empty);           // Q / dO row tiles are free once S^T and dP^T have retired
-        mbar_wait(&pds_full, i & 1);
-        mbar_wait(&qt_full, i & 1);
-        tc_fence_after();
-        const int q_valid = min(BT, p.nq - i * BT);
-        const int ksteps = (q_valid + 15) >> 4;
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint64_t ap = make_desc_sw128(smem_u32(sPt + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bo = make_desc_sw128(smem_u32(sdOt + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem + C::B_DV_COL, ap, bo, idesc_o, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint64_t as = make_desc_sw128(smem_u32(sdSt + (kk >> 2) * 16384)) + 2 * (kk & 3);
-          const uint64_t bq = make_desc_sw128(smem_u32(sQt + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
-          umma_bf16(tmem + C::B_DK_COL, as, bq, idesc_o, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&pds_empty);
-        umma_commit(&qt_empty);
-      }
-      umma_commit(&out_full);
-    }
-  } else {
-    const int r = warp * 32 + lane;
-    const uint32_t trow = tmem + (uint32_t(warp * 32) << 16);
-    const int key = k0 + r;
-    const bool row_ok = key < p.nk;
-    const int b = bh / p.heads, h = bh - b * p.heads;
-    int gsel = 0;   // 1: this key is the first concept-token column, 2: the second
-    if (p.gcols != nullptr) {
-      if (key == __ldg(p.pos + b * 2)) gsel = 1;
-      else if (key == __ldg(p.pos + b * 2 + 1)) gsel = 2;
-    }
-    for (int i = 0; i < T; ++i) {
-      const int buf = i & 1;
-      // stage lse / delta (/ probability-gradient columns) of this query tile in shared memory
-      for (int t = r; t < BT; t += 128) {
-        const int q = i * BT + t;
-        const bool ok = q < p.nq;
-        sL[buf][t] = ok ? __ldg(p.lse2 + (long long)bh * p.nq + q) : INFINITY;
-        sDl[buf][t] = ok ? __ldg(p.delta + (long long)bh * p.nq + q) : 0.f;
-        if (p.gcols != nullptr) {
-          sG0[buf][t] = ok ? __ldg(p.gcols + ((long long)b * p.nq + q) * 2) : 0.f;
-          sG1[buf][t] = ok ? __ldg(p.gcols + ((long long)b * p.nq + q) * 2 + 1) : 0.f;
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (lane == 0) {
-        mbar_wait(&stp_full, i & 1);
-        if (i > 0) mbar_wait(&pds_empty, (i - 1) & 1);
-      }
-      __syncwarp();
-      tc_fence_after();
-      const float* gp = gsel == 1 ? sG0[buf] : sG1[buf];
-#pragma unroll 1
-      for (int c = 0; c < BT / 32; ++c) {
-        uint32_t sv[32], dv[32];
-        tmem_ld32(trow + c * 32, sv);
-        tmem_ld32(trow + BT + c * 32, dv);
-        tmem_ld_wait();
-        float pr[32], ds[32];
-#pragma unroll
-        for (int k = 0; k < 32; ++k) {
-          const int col = c * 32 + k;
-          float e = ex2_approx_b(fmaf(__uint_as_float(sv[k]), p.scale_log2, -sL[buf][col]));
-          e = (row_ok && (!p.causal || key <= i * BT + col)) ? e : 0.f;
-          float dp = __uint_as_float(dv[k]);
-          if (gsel != 0) dp += gp[col];
-          pr[k] = e;
-          ds[k] = e * (dp - sDl[buf][col]) * p.scale;
-        }
-        store_row32_sw128(sPt, r, c, pr);
-        store_row32_sw128(sdSt, r, c, ds);
-      }
-      tc_fence_before();
-      mbar_arrive(&stp_empty);
-      fence_proxy_async_smem();
-      mbar_arrive(&pds_full);
-    }
-    if (lane == 0) mbar_wait(&out_full, 0);
-    __syncwarp();
-    tc_fence_after();
-    __nv_bfloat16* krow = p.dk + ((long long)b * p.nk + key) * p.lddk + h * D;
-    __nv_bfloat16* vrow = p.dv + ((long long)b * p.nk + key) * p.lddv + h * D;
-#pragma unroll 1
-    for (int c = 0; c < C::DV / 16; ++c) {
-      uint32_t vk[16], vv[16];
-      tmem_ld16(trow + C::B_DK_COL + c * 16, vk);
-      tmem_ld16(trow + C::B_DV_COL + c * 16, vv);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c * 16 + g * 8 < D) {
-            uint4 u, w;
-            u.x = pack_bf16x2(__uint_as_float(vk[g * 8 + 0]), __uint_as_float(vk[g * 8 + 1]));
-            u.y = pack_bf16x2(__uint_as_float(vk[g * 8 + 2]), __uint_as_float(vk[g * 8 + 3]));
-            u.z = pack_bf16x2(__uint_as_float(vk[g * 8 + 4]), __uint_as_float(vk[g * 8 + 5]));
-            u.w = pack_bf16x2(__uint_as_float(vk[g * 8 + 6]), __uint_as_float(vk[g * 8 + 7]));
-            w.x = pack_bf16x2(__uint_as_float(vv[g * 8 + 0]), __uint_as_float(vv[g * 8 + 1]));
-            w.y = pack_bf16x2(__uint_as_float(vv[g * 8 + 2]), __uint_as_float(vv[g * 8 + 3]));
-            w.z = pack_bf16x2(__uint_as_float(vv[g * 8 + 4]), __uint_as_float(vv[g * 8 + 5]));
-            w.w = pack_bf16x2(__uint_as_float(vv[g * 8 + 6]), __uint_as_float(vv[g * 8 + 7]));
-            *reinterpret_cast<uint4*>(krow + c * 16 + g * 8) = u;
-            *reinterpret_cast<uint4*>(vrow + c * 16 + g * 8) = w;
-          }
+        tma_load_3d(sQt, &tmQt, &q_full[st], i * BT, 0, bh);
+        tma_load_3d(sdOt, &tmdOt, &q_full[st], i * BT, 0, bh);
+        if (++st == C::STAGES) {
+          st = 0;
+          ph ^= 1;
         }
       }
     }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::B_TMEM);
+
+  const int wg = warp >> 2;
+  const int rA = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // key rows rA, rA + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  const int b = bh / p.heads, h = bh - b * p.heads;
+  int gsel[2] = {0, 0};   // 1: this key is the first concept-token column, 2: the second
+  if (p.gcols != nullptr) {
+    const int pos0 = __ldg(p.pos + b * 2), pos1 = __ldg(p.pos + b * 2 + 1);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int key = k0 + rA + 8 * hr;
+      gsel[hr] = key == pos0 ? 1 : (key == pos1 ? 2 : 0);
+    }
+  }
+  float dk[NO], dv[NO];
+#pragma unroll
+  for (int i = 0; i < NO; ++i) dk[i] = dv[i] = 0.f;
+  mbar_wait(&kv_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int i = 0; i < T; ++i) {
+    uint8_t* sQ = sStages + st * C::B_STAGE;
+    uint8_t* sdO = sQ + C::B_Q_BYTES;
+    uint8_t* sQt = sdO + C::B_Q_BYTES;
+    uint8_t* sdOt = sQt + C::B_QT_BYTES;
+    mbar_wait(&q_full[st], ph);
+    float s[NS], dp[NS];
+#pragma unroll
+    for (int x = 0; x < NS; ++x) s[x] = dp[x] = 0.f;
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    wgmma_fence();
+    bwd_rows_product<D, BT>(s, sK + wg * (64 * 128), sQ);
+    bwd_rows_product<D, BT>(dp, sV + wg * (64 * 128), sdO);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    const int q_valid = min(BT, p.nq - i * BT);
+    // per query column of this thread: lse, delta, probability gradient
+#pragma unroll
+    for (int c8 = 0; c8 < BT / 8; ++c8)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = 8 * c8 + cq + e, q = i * BT + col;
+        const bool ok = col < q_valid;
+        const float lq = ok ? __ldg(p.lse2 + (long long)bh * p.nq + q) : INFINITY;
+        const float dq = ok ? __ldg(p.delta + (long long)bh * p.nq + q) : 0.f;
+        float gq[2] = {0.f, 0.f};
+        if (p.gcols != nullptr && ok) {
+          gq[0] = __ldg(p.gcols + ((long long)b * p.nq + q) * 2);
+          gq[1] = __ldg(p.gcols + ((long long)b * p.nq + q) * 2 + 1);
+        }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int key = k0 + rA + 8 * hr;
+          const int x = 4 * c8 + 2 * hr + e;
+          float pr = ex2_approx_b(fmaf(s[x], p.scale_log2, -lq));
+          pr = (key < p.nk && (!p.causal || key <= q)) ? pr : 0.f;
+          float d = dp[x];
+          if (gsel[hr] != 0) d += gq[gsel[hr] - 1];
+          s[x] = pr;                              // P^T
+          dp[x] = pr * (d - dq) * p.scale;        // dS^T
+        }
+      }
+    const int ksteps = (q_valid + 15) >> 4;
+    const uint32_t zoff = (uint32_t)(z * C::DVH * 128);
+    wgmma_fence_regs(dk);
+    wgmma_fence_regs(dv);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BT / 16; ++kk) {
+      if (kk < ksteps) {
+        uint32_t a[4];
+        frag_to_a<false>(&s[8 * kk], a);
+        wgmma_rs<C::DVH, false>(dv, a, make_desc_sw128(smem_u32(sdOt) + zoff) + 2 * kk, 1u);
+        frag_to_a<false>(&dp[8 * kk], a);
+        wgmma_rs<C::DVH, false>(dk, a, make_desc_sw128(smem_u32(sQt) + zoff) + 2 * kk, 1u);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dk);
+    wgmma_fence_regs(dv);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&q_empty[st]);
+    if (++st == C::STAGES) {
+      st = 0;
+      ph ^= 1;
+    }
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int key = k0 + rA + 8 * hr;
+    if (key >= p.nk) continue;
+    __nv_bfloat16* krow = p.dk + ((long long)b * p.nk + key) * p.lddk + h * D + z * C::DVH;
+    __nv_bfloat16* vrow = p.dv + ((long long)b * p.nk + key) * p.lddv + h * D + z * C::DVH;
+#pragma unroll
+    for (int c8 = 0; c8 < C::DVH / 8; ++c8) {
+      const int col = 8 * c8 + cq;
+      if (z * C::DVH + col < D) {
+        *reinterpret_cast<uint32_t*>(krow + col) = pack_bf16x2(dk[4 * c8 + 2 * hr], dk[4 * c8 + 2 * hr + 1]);
+        *reinterpret_cast<uint32_t*>(vrow + col) = pack_bf16x2(dv[4 * c8 + 2 * hr], dv[4 * c8 + 2 * hr + 1]);
+      }
+    }
   }
 }
 
@@ -530,13 +446,13 @@ static int launch_bwd(const void* Q, const void* K, const void* V, const void* d
   int rc;
   if ((rc = rows_tmap(&tQa, Q, C::DP, p.nq, BH, 128))) return rc;
   if ((rc = rows_tmap(&tdOa, dO, C::DP, p.nq, BH, 128))) return rc;
-  if ((rc = rows_tmap(&tKa, K, C::DP, p.nk, BH, C::BTA))) return rc;
-  if ((rc = rows_tmap(&tVa, V, C::DP, p.nk, BH, C::BTA))) return rc;
+  if ((rc = rows_tmap(&tKa, K, C::DP, p.nk, BH, C::BT))) return rc;
+  if ((rc = rows_tmap(&tVa, V, C::DP, p.nk, BH, C::BT))) return rc;
   if ((rc = trans_tmap(&tKt, Kt, C::DV, nk8, BH))) return rc;
   if ((rc = rows_tmap(&tKb, K, C::DP, p.nk, BH, 128))) return rc;
   if ((rc = rows_tmap(&tVb, V, C::DP, p.nk, BH, 128))) return rc;
-  if ((rc = rows_tmap(&tQb, Q, C::DP, p.nq, BH, C::BTB))) return rc;
-  if ((rc = rows_tmap(&tdOb, dO, C::DP, p.nq, BH, C::BTB))) return rc;
+  if ((rc = rows_tmap(&tQb, Q, C::DP, p.nq, BH, C::BT))) return rc;
+  if ((rc = rows_tmap(&tdOb, dO, C::DP, p.nq, BH, C::BT))) return rc;
   if ((rc = trans_tmap(&tQt, Qt, C::DV, nq8, BH))) return rc;
   if ((rc = trans_tmap(&tdOt, dOt, C::DV, nq8, BH))) return rc;
   static bool configured = false;
@@ -545,10 +461,10 @@ static int launch_bwd(const void* Q, const void* K, const void* V, const void* d
     MOS_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::B_SMEM));
     configured = true;
   }
-  MOS_CHECK_CUDA(launch_pdl(attn_bwd_dq_kernel<D>, dim3((unsigned)ceil_div(p.nq, 128), (unsigned)BH), dim3(192),
+  MOS_CHECK_CUDA(launch_pdl(attn_bwd_dq_kernel<D>, dim3((unsigned)ceil_div(p.nq, 128), (unsigned)BH), dim3(BWD_THREADS),
                             (size_t)C::A_SMEM, stream, tQa, tdOa, tKa, tVa, tKt, p));
-  MOS_CHECK_CUDA(launch_pdl(attn_bwd_dkv_kernel<D>, dim3((unsigned)ceil_div(p.nk, 128), (unsigned)BH), dim3(192),
-                            (size_t)C::B_SMEM, stream, tKb, tVb, tQb, tdOb, tQt, tdOt, p));
+  MOS_CHECK_CUDA(launch_pdl(attn_bwd_dkv_kernel<D>, dim3((unsigned)ceil_div(p.nk, 128), (unsigned)BH, (unsigned)C::ZSPLIT),
+                            dim3(BWD_THREADS), (size_t)C::B_SMEM, stream, tKb, tVb, tQb, tdOb, tQt, tdOt, p));
   return MOS_OK;
 }
 

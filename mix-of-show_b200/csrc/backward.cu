@@ -292,7 +292,7 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, int DP, 
 //   step 2  thread (row group g of 4, lane) owns an 8-column chunk of x (-> dD) or dY (-> dU): one 128-bit load and 32
 //           FMAs per row; the 4 row groups are summed in a fixed order through smem
 // and writes its partial [4K + 4N]; lora_grad_reduce_kernel sums the <= 128 partials in a fixed order (bitwise
-// reproducible).  (The first version spent 16.6 ms of a 49.7 ms training step here; profiles/README.md.)
+// reproducible).
 constexpr int LG_THREADS = 256;
 constexpr int LG_MAX_BLOCKS = 128;
 

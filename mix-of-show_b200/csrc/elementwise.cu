@@ -334,7 +334,7 @@ __global__ void clip_embed_bwd_kernel(const int* __restrict__ ids, const __nv_bf
 }
 
 // ---------------------------------------------------------------------------------- VAE glue (AutoencoderKL)
-// Row softmax of fp32 logits (single-head d = 512 attention of the VAE mid block, computed as two tcgen05 GEMMs around this
+// Row softmax of fp32 logits (single-head d = 512 attention of the VAE mid block, computed as two wgmma GEMMs around this
 // kernel): out[r, c] = softmax_c(scale * S[r, c]) for c < cols, as 16-bit.  One warp per row, two passes over the row
 // (it is L2 resident: the producing GEMM has just written it).
 template <bool F16>

@@ -6,7 +6,7 @@
 // per-concept Gram matrices  G_c = X_c^T X_c:
 //     f(W) = s * sum_c tr((W - W_c) G_c (W - W_c)^T),   s = 1 / (n * out)
 //     grad = 2 s (W G - C),  G = sum_c G_c,  C = sum_c W_c G_c,   f = s (<W, W G - 2 C> + vv),  vv = sum_c <W_c, W_c G_c>
-// so features are reduced to [in, in] fp32 on the fly (tcgen05 GEMM with fp32 accumulate output, see gemm.cu) and a
+// so features are reduced to [in, in] fp32 on the fly (wgmma GEMM with fp32 accumulate output, see gemm.cu) and a
 // closure is one [out, in] x [in, in] fp32 GEMM.  Kernels here: bf16 transpose (Gram operand), small-n Gram, fp32
 // SGEMM, closure epilogue (grad + loss), deterministic vector primitives for the L-BFGS driver, batched LoRA merge.
 #include <stdlib.h>
@@ -456,7 +456,7 @@ extern "C" int mos_dgemm_mixed(const float* A, const double* B, double* C, int32
     tile_env = v;
   }
   int tile = tile_env;
-  if (tile == 0) tile = 2;   // 64 x 64: best under concurrent solves (config 3 A/B: 2.16 s vs 2.76 s (32 x 64) and 2.26 s (64 x 128))
+  if (tile == 0) tile = 2;   // 64 x 64 by default
   if (tile == 1) {
     dim3 grid((unsigned)ceil_div(N, 64), (unsigned)ceil_div(M, 32));
     dgemm_mixed_kernel<32, 64><<<grid, 256, smem(32, 64), STREAM(stream)>>>(A, B, C, M, N, K);
@@ -643,7 +643,7 @@ extern "C" int mos_lbfgs_direction_ring(const float* S_ring, const float* Y_ring
 
 extern "C" int mos_lora_merge(const int64_t* table_dev, int32_t n_layers, float alpha, void* stream) {
   MOS_CHECK_ARG(table_dev && n_layers > 0, "mos_lora_merge: bad arguments");
-  dim3 grid(148, (unsigned)n_layers);
+  dim3 grid(132, (unsigned)n_layers);   // one block row per SM of an H100 (the kernel strides over the layer)
   lora_merge_kernel<<<grid, 256, 0, STREAM(stream)>>>(reinterpret_cast<const long long*>(table_dev), alpha);
   MOS_CHECK_LAUNCH();
   return MOS_OK;

@@ -708,9 +708,12 @@ extern "C" int mos_groupnorm_fwd(const void* x, int64_t ldx, int32_t B, int32_t 
     int k = 1;
     static int min_ctas = 0;
     if (min_ctas == 0) {
+      int dev = 0, sms = 0;
+      MOS_CHECK_CUDA(cudaGetDevice(&dev));
+      MOS_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
       const char* e = getenv("MOS_GN_MIN_CTAS");      // clusters are widened until the grid has at least this many CTAs
-      min_ctas = e ? atoi(e) : 296;                  // two CTAs per SM: 6.10 vs 6.23 ms per step with 148 (profiles/README.md)
-      if (min_ctas < 1) min_ctas = 296;
+      min_ctas = e ? atoi(e) : 2 * sms;              // two CTAs per SM
+      if (min_ctas < 1) min_ctas = 2 * sms;
     }
     while (k < 8 && HW / (2 * k) >= 16 && (slab / k > 48 * 1024 || (long long)B * GN_GROUPS * k < min_ctas)) k *= 2;
     const int rows_per_cta = (int)ceil_div(HW, k);

@@ -1,5 +1,5 @@
-// tc.cuh — sm_100a primitives used by every tensor-core kernel in this library:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), UMMA descriptors.
+// tc.cuh — sm_90a primitives used by every tensor-core kernel in this library:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma descriptors (wgmma.cuh holds the MMA wrappers).
 // Inline PTX only; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -7,6 +7,8 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace mos {
 
@@ -26,8 +28,8 @@ __device__ __forceinline__ bool elect_one() {
 
 // ------------------------------------------------------------------ programmatic dependent launch (PDL)
 // Every kernel of the library is launched with cudaLaunchAttributeProgrammaticStreamSerialization: it may start while
-// its predecessor in the stream is still running, does its private prologue (smem carve-up, barrier init, TMEM
-// allocation), then pdl_wait() blocks until the predecessor has completed and flushed its writes.
+// its predecessor in the stream is still running, does its private prologue (smem carve-up, barrier init), then
+// pdl_wait() blocks until the predecessor has completed and flushed its writes.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -41,7 +43,7 @@ __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (UMMA / TMA reads)
+  // make generic-proxy smem writes visible to the async proxy (wgmma / TMA reads)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -76,9 +78,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // try_wait with a suspend-time hint: the hardware may park the thread (no issue slots used) until the phase completes
-// or `ns` nanoseconds pass.  A plain try_wait returns after ~50 cycles on B200, so a polling single-thread role
-// (TMA producer, MMA issuer) otherwise burns ~15 % of its scheduler's issue slots next to the busy softmax warps
-// (ncu source view of the attention kernel: profiles/README.md).
+// or `ns` nanoseconds pass, so that a polling single-thread role (the TMA producer) does not take issue slots from the
+// math warps it shares a scheduler with.
 __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t ns) {
   uint32_t ok;
   asm volatile(
@@ -163,116 +164,18 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> f32, one CTA
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, tf32 inputs (fp32 storage, 10-bit mantissa used)
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// same, arriving on the mbarrier at this smem offset in every CTA of the cluster selected by `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive fp32 columns: thread t of the warp gets row (lane base + t)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns written back to TMEM (thread t of the warp owns row lane base + t)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(
-          taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ UMMA descriptors
-// K-major operand tile in shared memory, rows of 64 bf16 (=128 B), SWIZZLE_128B, 8-row groups 1024 B apart.
-// (cute/arch/mma_sm100_desc.hpp SmemDescriptor: start[0,14) LBO[16,30) SBO[32,46) version[46,48)=1 layout[61,64)=2)
+// ------------------------------------------------------------------ wgmma shared-memory descriptor
+// K-major operand tile in shared memory, rows of 64 16-bit elements (=128 B), SWIZZLE_128B, 8-row groups 1024 B apart
+// (sm_90 matrix descriptor: start[0,14) LBO[16,30) SBO[32,46) base offset[49,52) layout[62,64) = 1 for SWIZZLE_128B).
+// The tile must start on a 1024-byte boundary; +2 in the start field advances 16 elements (32 B) along K inside the atom.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>(1) << 16;            // LBO (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;            // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;            // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16 / kind::tf32, fp32 accumulate, both operands K-major.
-// fmt: 0 = f16, 1 = bf16, 2 = tf32
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int fmt) {
-  return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(N >> 3) << 17) |
-         (uint32_t(M >> 4) << 24);
-}
-// (The descriptor has separate A / B format fields, but B200 faults - illegal instruction - on a kind::f16 MMA whose two
-// formats differ, measured in round 2; both operands therefore always share `fmt`.)
 
 // ------------------------------------------------------------------ small math helpers
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
@@ -284,7 +187,7 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(t);
 }
 // 16-bit storage (activations and packed weights) is bf16 (training) or fp16 (sampling: 3 more mantissa bits, which is what
-// keeps the classifier-free-guidance difference c - u accurate; profiles/README.md "numerics, round 2"); F16 = the codec.
+// keeps the classifier-free-guidance difference c - u accurate); F16 = the codec.
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   __half2 t = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&t);
@@ -310,6 +213,14 @@ template <bool F16>
 __device__ __forceinline__ float ld16(const __nv_bfloat16* p) {   // 16-bit storage is typed __nv_bfloat16* throughout
   const uint16_t u = *reinterpret_cast<const uint16_t*>(p);
   return F16 ? __half2float(__ushort_as_half(u)) : __bfloat162float(__ushort_as_bfloat16(u));
+}
+// Accumulator fragment (wgmma.cuh) of columns [16k, 16k + 16), d = &acc[8k] -> the A register fragment of one k16 step
+template <bool F16>
+__device__ __forceinline__ void frag_to_a(const float* d, uint32_t (&a)[4]) {
+  a[0] = pack16x2<F16>(d[0], d[1]);
+  a[1] = pack16x2<F16>(d[2], d[3]);
+  a[2] = pack16x2<F16>(d[4], d[5]);
+  a[3] = pack16x2<F16>(d[6], d[7]);
 }
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + __expf(-x)); }

@@ -1,4 +1,4 @@
-"""B200 gradient fusion — drop-in for the UNet half of the reference's `gradient_fusion.py`.
+"""GPU gradient fusion — drop-in for the UNet half of the reference's `gradient_fusion.py`.
 
   update_quasi_newton(K_target, V_target, W, iters, device)     <- gradient_fusion.py:38-96 (+ chunk_compute_mse :22-35)
   merge_lora_into_weight(original, lora, layer_names, model_type, alpha, device)   <- :99-143
@@ -8,11 +8,11 @@
 Design (DESIGN.md §4, fusion.cu header): the per-layer objective  mean((X W^T - V)^2)  depends on the recorded
 features only through G = X^T X and C = V^T X.  The reference keeps X, V (GBs) in host RAM and re-streams them to the
 GPU for each of the <= 62 closure evaluations per layer; here the UNet engine reduces the features to per-concept
-Gram matrices on the fly (tcgen05 GEMM, fp32 accumulate), and a closure is one [out,in]x[in,in] fp32 GEMM.
+Gram matrices on the fly (wgmma GEMM, fp32 accumulate), and a closure is one [out,in]x[in,in] fp32 GEMM.
 The optimiser is the same algorithm the reference calls (torch.optim.LBFGS: history 25, lr 1, strong-Wolfe line
 search, tolerance 1e-16, ONE .step of max_iter iterations, best iterate over all closure evaluations), restated here
 over CUDA vector primitives (mos_vec_*), working on the correction D = W - W0 so that the quadratic is evaluated
-without the cancellation of the raw Gram form.  The text-encoder half (merge_text_encoder) runs on the B200 CLIP engine
+without the cancellation of the raw Gram form.  The text-encoder half (merge_text_encoder) runs on the GPU CLIP engine
 (mos_b200/clip_engine.py).  The reference's entry point (parse_new_concepts, merge_new_concepts_, get_text_feature,
 compose_concepts and the CLI) is restated at the bottom of this file over those stages.
 """
@@ -434,7 +434,7 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
     """Text-encoder fusion (gradient_fusion.py:460-565).  text_encoder_list[c]: concept c's CLIP LoRA
     ({'text_model.encoder.layers.{i}.self_attn.{q,k,v,out}_proj.lora_{down,up}.weight'}); prompt_ids[c]: the un-padded
     token-id sequences of concept c's 32 layer-bound prompts ('photo of a <c>' and '<c>' x 16, :515-520; the tokenizer
-    runs upstream).  For every concept its LoRA is merged (:505-512), the prompts run through the B200 CLIP engine and
+    runs upstream).  For every concept its LoRA is merged (:505-512), the prompts run through the GPU CLIP engine and
     the inputs of the LoRA'd linears at ALL valid token positions are recorded (the reference's forward hooks, :146-167,
     :525-541); every layer is then solved from the accumulated Gram matrices as in merge_kv_in_cross_attention.
     Causal attention makes the features of a valid position independent of the padding behind it, so the sequences are
@@ -485,7 +485,7 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
 class GramRecorder:
     """Engine-side replacement of the reference's forward hooks (gradient_fusion.py:146-167): instead of copying
     every (input, output - bias) pair to host RAM, accumulate G += X^T X per recorded GEMM input on the tensor
-    cores (transpose -> tcgen05 GEMM with fp32 accumulate output)."""
+    cores (transpose -> wgmma GEMM with fp32 accumulate output)."""
 
     def __init__(self, device):
         self.dev, self.G, self.rows, self._xt = device, {}, {}, {}
@@ -618,7 +618,7 @@ def _check_lora_targets(params, path):
     bad += [k for k in (params.get('text_encoder') or {}) if not k.endswith(_TEXT_LORA_SUFFIXES)]
     if bad:
         raise ValueError(f'{path}: unsupported LoRA target(s) {bad[:3]}{" ..." if len(bad) > 3 else ""}: gradient fusion on '
-                         'the B200 path handles attention-projection LoRA (where: Attention / CLIPAttention) only')
+                         'the GPU path handles attention-projection LoRA (where: Attention / CLIPAttention) only')
 
 
 def parse_new_concepts(concept_cfg):
@@ -711,7 +711,7 @@ def cross_kv_layer_names(unet):
 
 def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, pretrained_model_path, save_path, suffix,
                      device='cuda', tokenizer=None, log=print):
-    """gradient_fusion.py:750-813 on the B200 path.  `pretrained_model_path`: diffusers-layout directory (unet/,
+    """gradient_fusion.py:750-813 on the GPU path.  `pretrained_model_path`: diffusers-layout directory (unet/,
     text_encoder/, tokenizer/); the fused UNet / text encoder and new_concept_cfg.json are written to
     `{save_path}/combined_model_{suffix}` together with the tokenizer that carries the added `<new{k}>` tokens (the VAE /
     scheduler folders of the base model are untouched by the fusion and are not copied here)."""

@@ -1,5 +1,5 @@
 """Drop-in for the reference's `mixofshow/models/edlora.py` (same names, argument meaning and error behaviour), with
-the arithmetic executed by hand-written sm_100a kernels (libmos_sm100.so) instead of diffusers / xformers / cuBLAS.
+the arithmetic executed by hand-written sm_90a kernels (libmos_sm100.so) instead of diffusers / xformers / cuBLAS.
 
   LoRALinearLayer                                   <- mixofshow/models/edlora.py:221-246
   EDLoRA_AttnProcessor                              <- :103-173
@@ -11,7 +11,7 @@ the arithmetic executed by hand-written sm_100a kernels (libmos_sm100.so) instea
 Two ways these objects are used:
   * operator level (exactly the reference protocol): `processor(attn, hidden_states, encoder_hidden_states=...)`
     and `module(x)` on a LoRA-patched module run the fused CUDA kernels on the tensors they are given;
-  * whole-UNet level: the B200 UNet (`mixofshow.models.unet_b200.UNet2DConditionModel`) reads them as descriptors
+  * whole-UNet level: the GPU UNet (`mixofshow.models.unet_b200.UNet2DConditionModel`) reads them as descriptors
     (which layer index, which controller, which LoRA pairs) and configures the captured denoise step.
 """
 import math
@@ -160,13 +160,13 @@ def revise_edlora_unet_attention_controller_forward(unet, controller):
 
 class LoRALinearLayer(nn.Module):
     """y = original(x) + alpha * up(down(x)) on a Linear or 1x1 Conv2d, installed by overwriting the module's
-    forward exactly as the reference does; the forward is one fused tcgen05 GEMM (K1)."""
+    forward exactly as the reference does; the forward is one fused wgmma GEMM (K1)."""
 
     def __init__(self, name, original_module, rank=4, alpha=1):
         super().__init__()
         self.name = name
         if rank > 4:
-            raise ValueError('the fused sm_100a epilogue supports LoRA rank <= 4 (the reference default is 4)')
+            raise ValueError('the fused sm_90a epilogue supports LoRA rank <= 4 (the reference default is 4)')
         if original_module.__class__.__name__ == 'Conv2d':
             in_channels, out_channels = original_module.in_channels, original_module.out_channels
             self.lora_down = torch.nn.Conv2d(in_channels, rank, (1, 1), bias=False)

@@ -1,4 +1,4 @@
-"""B200 `UNet2DConditionModel`: the object the reference's entry points call as
+"""GPU `UNet2DConditionModel`: the object the reference's entry points call as
 `unet(sample, t, encoder_hidden_states=..., cross_attention_kwargs=..., down_block_additional_residuals=...).sample`
 (mixofshow/pipelines/pipeline_edlora.py:277, trainer_edlora.py:237, gradient_fusion.py:619,
 pipeline_regionally_t2iadapter.py:556).
@@ -22,7 +22,7 @@ SD15 = dict(in_channels=4, out_channels=4, block_out_channels=(320, 640, 1280, 1
 
 
 def _no_forward(self, *a, **k):
-    raise RuntimeError(f'{self.__class__.__name__}.forward is not executed on the B200 path: call the UNet '
+    raise RuntimeError(f'{self.__class__.__name__}.forward is not executed on the GPU path: call the UNet '
                        '(whole-step engine) or an attention processor (operator level) instead')
 
 
@@ -313,7 +313,7 @@ class UNet2DConditionModel(nn.Module):
     def forward(self, sample, timestep, encoder_hidden_states, cross_attention_kwargs=None,
                 down_block_additional_residuals=None, return_dict=True):
         if not sample.is_cuda:
-            raise RuntimeError('the B200 UNet needs CUDA tensors (there is no CPU fallback)')
+            raise RuntimeError('the GPU UNet needs CUDA tensors (there is no CPU fallback)')
         B, _, H, W = sample.shape
         sess = self.session(B, H, W, sample.device, encoder_hidden_states, cross_attention_kwargs,
                             down_block_additional_residuals)

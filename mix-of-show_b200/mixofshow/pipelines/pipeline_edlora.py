@@ -1,9 +1,9 @@
 """Drop-in for the reference's `mixofshow/pipelines/pipeline_edlora.py`: `bind_concept_prompt` and `EDLoRAPipeline`
 with the same constructor / `set_new_concept_cfg` / `set_controller` / `__call__` surface.
 
-The denoise loop (reference :271-301) runs on the B200 engine: per step one captured UNet graph (CFG batch 2) and
+The denoise loop (reference :271-301) runs on the GPU engine: per step one captured UNet graph (CFG batch 2) and
 ONE fused kernel for CFG combine + DPM-Solver++(2M) update + re-duplication of the latents (`mos_cfg_dpmpp_step`).
-Prompt encoding and image decoding run on the B200 CLIP / VAE engines (mixofshow/models/clip_b200.py, vae_b200.py) when
+Prompt encoding and image decoding run on the GPU CLIP / VAE engines (mixofshow/models/clip_b200.py, vae_b200.py) when
 `from_pretrained` finds `text_encoder/` and `vae/`; without them pass `prompt_embeds` and request `output_type='latent'`.
 """
 from types import SimpleNamespace
@@ -44,7 +44,7 @@ def bind_concept_prompt(prompts, new_concept_cfg):
 class EDLoRAPipeline:
     def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None, safety_checker=None,
                  feature_extractor=None, requires_safety_checker: bool = False):
-        assert unet is not None, 'EDLoRAPipeline needs the B200 UNet'
+        assert unet is not None, 'EDLoRAPipeline needs the GPU UNet'
         revise_edlora_unet_attention_forward(unet)          # reference :93
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.scheduler = scheduler if scheduler is not None else DPMSolverPP2M()
@@ -57,8 +57,8 @@ class EDLoRAPipeline:
     def from_pretrained(cls, pretrained_model_name_or_path, scheduler=None, vae=None, tokenizer=None, device='cuda',
                         **unused):
         """diffusers call shape (`EDLoRAPipeline.from_pretrained(path, scheduler=..., torch_dtype=...)`, test_edlora.py /
-        README.md:146): loads `unet/` and `text_encoder/` of a diffusers-layout directory into the B200 containers
-        (mixofshow/utils/model_io.py), `vae/` (when present) into the B200 VAE and `tokenizer/` through transformers."""
+        README.md:146): loads `unet/` and `text_encoder/` of a diffusers-layout directory into the GPU containers
+        (mixofshow/utils/model_io.py), `vae/` (when present) into the GPU VAE and `tokenizer/` through transformers."""
         import os
         from mixofshow.utils import model_io
         unet = model_io.load_unet(pretrained_model_name_or_path)

@@ -2,7 +2,7 @@
 `RegionT2I_AttnProcessor`, `revise_regionally_t2iadapter_attention_forward`, `RegionallyT2IAdapterPipeline`.
 
 The region-masked cross-attention (reference :32-86) runs as: one flash cross-attention per region with the region's
-own K/V (tcgen05), then `mos_region_combine` (global outside the boxes, mean of covering regions inside).  Box indices
+own K/V (wgmma), then `mos_region_combine` (global outside the boxes, mean of covering regions inside).  Box indices
 are computed on the host in Python float64 exactly as the reference does (`math.ceil` / `math.floor`), so they are
 bit-exact.  The T2I-Adapter networks themselves are out of scope (SURVEY.md §2.1 row 6): pass their four feature
 maps as `adapter_state` (or torch adapter modules as `keypose_adapter` / `sketch_adapter` attributes).
@@ -151,7 +151,7 @@ class RegionallyT2IAdapterPipeline:
                  generator=None, latents=None, prompt_embeds=None, negative_prompt_embeds=None, output_type='pil',
                  return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None,
                  region_list=None, keypose_adapter_state=None, sketch_adapter_state=None):
-        """Extra (B200) arguments: `region_list` = [(region_embeds [2,16,77,768], box fractions)] and
+        """Extra (GPU path) arguments: `region_list` = [(region_embeds [2,16,77,768], box fractions)] and
         `*_adapter_state` = precomputed T2I-Adapter feature maps (4 NCHW tensors), for use without CLIP / adapters."""
         device = self.device
         do_cfg = guidance_scale > 1.0

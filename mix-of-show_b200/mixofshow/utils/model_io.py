@@ -6,7 +6,7 @@
         <dir>/text_encoder/config.json + model.safetensors (or pytorch_model.bin)
   * `<dir>/new_concept_cfg.json` (`gradient_fusion.py:812-813`).
 
-`load_unet` / `load_text_encoder` build this repo's B200 containers from such a directory; `save_combined_model` writes
+`load_unet` / `load_text_encoder` build this repo's GPU containers from such a directory; `save_combined_model` writes
 one.  diffusers itself is not a dependency: the UNet `config.json` keys are the SD1.5 ones (diffusers 0.19.3), and any
 option this path does not implement is rejected loudly instead of being ignored."""
 import json
@@ -26,7 +26,7 @@ UNET_CONFIG_SD15 = {
     'mid_block_scale_factor': 1, 'norm_eps': 1e-05, 'norm_num_groups': 32, 'out_channels': 4, 'sample_size': 64,
     'up_block_types': ['UpBlock2D', 'CrossAttnUpBlock2D', 'CrossAttnUpBlock2D', 'CrossAttnUpBlock2D'],
 }
-# options that change the arithmetic: only these values are implemented by the B200 engine
+# options that change the arithmetic: only these values are implemented by the GPU engine
 _UNET_REQUIRED = {
     'act_fn': 'silu', 'center_input_sample': False, 'downsample_padding': 1, 'flip_sin_to_cos': True, 'freq_shift': 0,
     'mid_block_scale_factor': 1, 'norm_num_groups': 32, 'use_linear_projection': False, 'only_cross_attention': False,
@@ -54,10 +54,10 @@ def _write_weights(folder, name, state_dict):
 
 
 def check_unet_config(cfg):
-    """Reject diffusers UNet options the B200 engine does not implement (instead of silently ignoring them)."""
+    """Reject diffusers UNet options the GPU engine does not implement (instead of silently ignoring them)."""
     for k, want in _UNET_REQUIRED.items():
         if k in cfg and cfg[k] != want and not (want is False and cfg[k] is None):
-            raise ValueError(f'unet/config.json: {k}={cfg[k]!r} is not supported on the B200 path (needs {want!r})')
+            raise ValueError(f'unet/config.json: {k}={cfg[k]!r} is not supported on the GPU path (needs {want!r})')
     nb = len(cfg['block_out_channels'])
     down = cfg.get('down_block_types', ['CrossAttnDownBlock2D'] * (nb - 1) + ['DownBlock2D'])
     up = cfg.get('up_block_types', ['UpBlock2D'] + ['CrossAttnUpBlock2D'] * (nb - 1))
@@ -148,7 +148,7 @@ def load_vae(model_dir, subfolder='vae', device='cuda'):
         cfg = json.load(f)
     for k, want in _VAE_REQUIRED.items():
         if k in cfg and cfg[k] != want:
-            raise ValueError(f'vae/config.json: {k}={cfg[k]!r} is not supported on the B200 path (needs {want!r})')
+            raise ValueError(f'vae/config.json: {k}={cfg[k]!r} is not supported on the GPU path (needs {want!r})')
     down = cfg.get('down_block_types')
     if down is not None and any(t != 'DownEncoderBlock2D' for t in down):
         raise ValueError(f'unsupported VAE block layout {down}')

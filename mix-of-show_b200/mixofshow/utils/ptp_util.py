@@ -1,4 +1,4 @@
-"""Attention controllers with the reference's call protocol (mixofshow/utils/ptp_util.py:11-108): the B200 processors
+"""Attention controllers with the reference's call protocol (mixofshow/utils/ptp_util.py:11-108): the GPU processors
 hand them the cross-attention probability maps `[B*heads, N, 77]`.  Notebook visualisation helpers of the reference
 file are out of scope (SURVEY.md §2.1 row 8)."""
 import abc

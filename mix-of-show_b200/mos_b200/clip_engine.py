@@ -1,4 +1,4 @@
-"""CLIPTextEngine — the CLIP text encoder forward on B200 (SURVEY.md §8f rank 1), built only from libmos_sm100 kernels.
+"""CLIPTextEngine — the CLIP text encoder forward on the GPU (SURVEY.md §8f rank 1), built only from libmos_sm100 kernels.
 
 Owns the `text_encoder(input_ids)[0]` call the reference makes at mixofshow/pipelines/pipeline_edlora.py:133-145,
 trainer_edlora.py:220-234 and gradient_fusion.py:182-199 (transformers `CLIPTextModel`: token + position embeddings,

@@ -1,4 +1,4 @@
-"""CLIPTrainEngine — the text-encoder half of one ED-LoRA training step on B200: forward with saved activations and the
+"""CLIPTrainEngine — the text-encoder half of one ED-LoRA training step on the GPU: forward with saved activations and the
 backward that turns d(last_hidden_state) into the gradients of the NEW-CONCEPT EMBEDDING ROWS and of the CLIPAttention LoRA
 (`where: CLIPAttention`, q/k/v/out_proj of all 12 layers), built only from libmos_sm100 kernels.
 

@@ -1,4 +1,4 @@
-"""UNetEngine — the SD1.5 UNet + ED-LoRA denoising step on B200, built only from libmos_sm100 kernels.
+"""UNetEngine — the SD1.5 UNet + ED-LoRA denoising step on the GPU, built only from libmos_sm100 kernels.
 
 The engine owns the whole `unet(sample, t, encoder_hidden_states, cross_attention_kwargs,
 down_block_additional_residuals).sample` call the reference makes at
@@ -21,10 +21,11 @@ from ._lib import MOS_SEG_ROWS, MOS_SEG_TRANSPOSED
 BF16 = torch.bfloat16       # weights (and the training engine's activations)
 F16 = torch.float16
 # split-K GEMMs finalize in-kernel (mos_gemm_args.tile_counters); MOS_SPLITK_FUSED=0 restores the separate
-# mos_splitk_finalize launch (A/B timing, profiles/README.md)
+# mos_splitk_finalize launch (A/B timing)
 FUSED_SPLITK = os.environ.get('MOS_SPLITK_FUSED', '0') == '1'
 # every GEMM of the step stages the NEXT GEMM's weight matrix in L2 while it runs (mos_gemm_args.prefetch_ptr): the step
-# streams 1.7 GB of weights through a mostly idle HBM, the 126 MB L2 holds any single layer.  MOS_L2_PREFETCH=0/1.
+# streams 1.7 GB of weights through a mostly idle HBM, and the 50 MB L2 of an H100 holds any single layer (at most 48 MB
+# is staged).  MOS_L2_PREFETCH=0/1.
 L2_PREFETCH = os.environ.get('MOS_L2_PREFETCH', '0') == '1'
 L2_PREFETCH_MAX_BYTES = 48 << 20
 SPLITK_MIN_KB = int(os.environ.get('MOS_SPLITK_MIN_KB', '8'))      # fewest 64-deep k-blocks a split-K slice may get
@@ -56,11 +57,11 @@ class UNetEngine:
         """state_dict: diffusers-named fp32 tensors of the UNet.  lora: {f'{module}.lora_down.weight': [r,in],
         f'{module}.lora_up.weight': [out,r]} exactly as EDLoRATrainer.delta_state_dict()['unet'] stores it
         (trainer_edlora.py:371-378); rank <= 4.  batch includes the CFG duplication.  height/width: latent size.
-        act_dtype: 16-bit type of every activation AND of the packed GEMM weights (tcgen05 kind::f16 takes one operand
-        format per MMA).  Sampling uses fp16 - the reference's own sampling precision (README.md:146 torch_dtype=float16):
+        act_dtype: 16-bit type of every activation AND of the packed GEMM weights (wgmma takes one operand type for
+        A and B).  Sampling uses fp16 - the reference's own sampling precision (README.md:146 torch_dtype=float16):
         with classifier-free guidance the scheduler consumes u + g (c - u), so the activation rounding noise of the two
         (nearly equal) halves is amplified by g; fp16's 3 extra mantissa bits bring the CFG-7.5 latents from 2.8e-3 (bf16,
-        round 1) to < 5e-4 rel-L2 (tests/numerics_emulation.py, profiles/README.md).  Training keeps bf16 (gradient range)."""
+        round 1) to < 5e-4 rel-L2 (tests/numerics_emulation.py).  Training keeps bf16 (gradient range)."""
         assert act_dtype in (F16, BF16)
         self.ACT = act_dtype
         self.dev = torch.device(device)
@@ -275,7 +276,8 @@ class UNetEngine:
         tiles = _r(M, 128) // 128 * (N // 160)
         if tiles >= 96 or kb_total < 2 * SPLITK_MIN_KB:
             return 1
-        s = max(1, min(max(1, 148 // tiles), kb_total // SPLITK_MIN_KB, 16))
+        sms = torch.cuda.get_device_properties(self.dev).multi_processor_count   # the GEMM grid is one CTA per SM
+        s = max(1, min(max(1, sms // tiles), kb_total // SPLITK_MIN_KB, 16))
         per = -(-kb_total // s)          # k blocks per split
         return -(-kb_total // per)       # normalised so that no split is empty
 

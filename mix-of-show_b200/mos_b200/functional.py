@@ -44,7 +44,7 @@ def pack_linears(modules, device):
     W = torch.cat(Ws, 0)
     N, K = W.shape
     if N % 160 != 0 or K % 64 != 0:
-        raise ValueError(f'unsupported projection shape [{N}, {K}]: the sm_100a GEMM needs N % 160 == 0 and K % 64 == 0')
+        raise ValueError(f'unsupported projection shape [{N}, {K}]: the sm_90a GEMM needs N % 160 == 0 and K % 64 == 0')
     ent = {'N': N, 'K': K, 'W': W.to(ACT).contiguous(), 'bias': None}
     if any(b is not None for b in bs):
         ent['bias'] = torch.cat([b if b is not None else torch.zeros(w.shape[0], device=device)
@@ -89,9 +89,9 @@ def _lora_kw(ent):
 
 def lora_linear(module, x):
     """y = module(x) + alpha * up(down(x))  — LoRALinearLayer.forward (mixofshow/models/edlora.py:244-246) as one
-    fused tcgen05 GEMM.  module: nn.Linear or 1x1 nn.Conv2d carrying a `_mos_lora` descriptor (or none)."""
+    fused wgmma GEMM.  module: nn.Linear or 1x1 nn.Conv2d carrying a `_mos_lora` descriptor (or none)."""
     if not x.is_cuda:
-        raise ValueError('the B200 path needs CUDA tensors (there is no CPU fallback)')
+        raise ValueError('the GPU path needs CUDA tensors (there is no CPU fallback)')
     ent = _cached(module, 'self', [module], x.device)
     conv = module.__class__.__name__ == 'Conv2d'
     if conv:
@@ -115,7 +115,7 @@ def attention_block(attn, hidden_states, encoder_hidden_states=None, want_probs=
     (region_embeds [B, M, Cc], (sh, sw, eh, ew) feature-pixel ints) for the regional rewrite.
     Returns (out [B, N, C] in hidden_states.dtype, probs fp32 [B*heads, N, M] or None)."""
     if not hidden_states.is_cuda:
-        raise ValueError('the B200 path needs CUDA tensors (there is no CPU fallback)')
+        raise ValueError('the GPU path needs CUDA tensors (there is no CPU fallback)')
     dev = hidden_states.device
     B, N, C = hidden_states.shape
     Hh = attn.heads

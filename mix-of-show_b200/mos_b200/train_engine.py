@@ -1,4 +1,4 @@
-"""TrainEngine — the UNet side of one ED-LoRA training step on B200 (EDLoRATrainer.forward from `add_noise` to the
+"""TrainEngine — the UNet side of one ED-LoRA training step on the GPU (EDLoRATrainer.forward from `add_noise` to the
 loss, trainer_edlora.py:218-261, the `loss.backward()` of train_edlora.py:120-123 and the AdamW update of the UNet LoRA
 group, train_edlora.py:57,129), built only from libmos_sm100 kernels.
 

@@ -1,4 +1,4 @@
-"""VAEEngine — the SD1.5 `AutoencoderKL` encoder and decoder on B200 (SURVEY.md 8f rank 2), built only from libmos_sm100
+"""VAEEngine — the SD1.5 `AutoencoderKL` encoder and decoder on the GPU (SURVEY.md 8f rank 2), built only from libmos_sm100
 kernels.  Owns the two calls the reference makes:
 
     latents = self.vae.encode(images).latent_dist.sample() * 0.18215     mixofshow/pipelines/trainer_edlora.py:203-204
@@ -11,7 +11,7 @@ asymmetric-padded stride-2 downsampling, nearest x2 upsampling).  Activations ar
 Shapes are bent to the GEMM kernel's 160-column tiles without touching the arithmetic: a C-channel tensor lives in a
 [M, Cp] buffer (Cp = C rounded up to 160: 128 -> 160, 256 -> 320, 512 -> 640) whose pad columns are written as zeros (zero
 weight rows, zero bias); reductions run over the C real channels (pixel pitch Cp).  The d = 512 attention is
-S = Q K^T (tcgen05 GEMM, fp32 out) -> mos_softmax_rows -> O = P V (tcgen05 GEMM): the 4096 x 4096 logits of a 512^2 image
+S = Q K^T (wgmma GEMM, fp32 out) -> mos_softmax_rows -> O = P V (wgmma GEMM): the 4096 x 4096 logits of a 512^2 image
 are 68 MB, once per image.  No CPU / PyTorch fallback: every arithmetic op is a C-ABI call.
 """
 import torch

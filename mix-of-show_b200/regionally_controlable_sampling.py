@@ -1,4 +1,4 @@
-"""B200 mirror of the reference's `regionally_controlable_sampling.py` entry script (BASELINE config 4): region-string
+"""GPU mirror of the reference's `regionally_controlable_sampling.py` entry script (BASELINE config 4): region-string
 parsing, model loading from a fused `combined_model_*` directory, and the sampling call.  Host logic only; the UNet loop runs
 on `RegionallyT2IAdapterPipeline` (mixofshow/pipelines/pipeline_regionally_t2iadapter.py).
 

@@ -1,4 +1,4 @@
-"""B200 mirror of the reference training entry point (train_edlora.py): `python train_edlora.py -opt <yml>` ->
+"""GPU mirror of the reference training entry point (train_edlora.py): `python train_edlora.py -opt <yml>` ->
 `EDLoRATrainer(**opt['models'])` -> the loop of train_edlora.py:105-158.
 
 One process per GPU (launch with torchrun for data parallelism), the batch sharded across ranks, ONE NCCL all-reduce per

@@ -11,7 +11,7 @@ for p in (ROOT, PKG):  # PKG also exposes the top-level gradient_fusion module
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100; select with -m gpu)')
 
 
 @pytest.fixture(scope='session')

@@ -1,9 +1,9 @@
 """Numerics experiment on the fp32 CPU oracle (test infrastructure; not collected by pytest, not a product path).
 
-Emulates WHERE the B200 engine rounds (GEMM operands, weights, stored intermediates, the residual stream) by running
+Emulates WHERE the GPU engine rounds (GEMM operands, weights, stored intermediates, the residual stream) by running
 the oracle UNet with rounding functions inserted at the same points, and prints the eps error and the post-scheduler
 latent error (guidance 1 and 7.5) against the un-rounded fp32 oracle.  It answered the round-2 design question "what has
-to stay fp32 for the CFG-7.5 latents to meet 1e-3": see profiles/README.md (numerics table, round 2).
+to stay fp32 for the CFG-7.5 latents to meet 1e-3" (answer: fp16 operands; see DESIGN.md "Numerics").
 
     python tests/numerics_emulation.py [--full] [--modes a,b,...]
 """

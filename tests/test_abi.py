@@ -41,8 +41,8 @@ def test_argument_validation_without_gpu():
     assert rc == -1 and b'act_dtype' in lib.mos_last_error()
 
 
-def test_sass_is_blackwell_native():
-    """SASS of the built library must contain tcgen05 (UTC*MMA), TMEM loads (LDTM) and TMA (UTMALDG)."""
+def test_sass_is_hopper_native():
+    """SASS of the built library must contain sm_90a warpgroup MMAs (HGMMA) and TMA (UTMALDG)."""
     import shutil
     import subprocess
     cuobjdump = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
@@ -51,5 +51,5 @@ def test_sass_is_blackwell_native():
         pytest.skip('cuobjdump not available')
     lib_path = _build()
     sass = subprocess.run([cuobjdump, '-sass', lib_path], capture_output=True, text=True).stdout
-    assert 'UTCHMMA' in sass and 'LDTM' in sass and 'UTMALDG' in sass
-    assert 'HMMA.' not in sass.replace('UTCHMMA', ''), 'legacy mma.sync path found'
+    assert 'arch = sm_90a' in sass and 'HGMMA' in sass and 'UTMALDG' in sass
+    assert 'HMMA.' not in sass, 'legacy mma.sync path found'

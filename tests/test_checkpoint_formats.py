@@ -1,12 +1,12 @@
 """On-disk / checkpoint plumbing (SURVEY.md 8f rank 3), CPU only: the ED-LoRA delta checkpoint layout
 (trainer_edlora.py:358-378, train_edlora.py:168-171) loaded through this repo's `convert_edlora_to_diffusers` mirror into
-this repo's containers, cross-checked live against the reference's own file where /root/reference exists."""
+this repo's containers, cross-checked against what the reference's own file computes (stored golden data)."""
 import io
 
 import pytest
 import torch
 
-from oracle import inject, ref_shims
+from oracle import inject
 from oracle import unet as ou
 
 
@@ -125,29 +125,31 @@ def test_clip_container_embedding_surface(monkeypatch):
         te.load_state_dict({'nope': torch.zeros(1)})
 
 
-@pytest.mark.skipif(not ref_shims.reference_available(), reason='reference checkout not present')
-def test_mirror_matches_reference_file_live():
+def test_mirror_matches_reference_file():
+    """This repo's convert_edlora_to_diffusers mirror against what the reference's own file computed on the same seeded
+    checkpoint (tests/golden/reference_live.pt, generated by tests/golden/make_reference_live.py)."""
+    import os
     from types import SimpleNamespace
     from mixofshow.utils import convert_edlora_to_diffusers as mine
-    ref = ref_shims.load_reference_module('mixofshow/utils/convert_edlora_to_diffusers.py')
+    L = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_live.pt'),
+                   weights_only=False)
     unet = ou.build_unet(0, ou.TINY)
     clip, clip_sd = _clip_sd()
     ckpt = _delta(unet, clip, seed=5)['params']
     for model_type, sd in (('unet', unet.state_dict()), ('text_encoder', clip_sd)):
-        a = ref.merge_lora_into_weight(sd, ckpt[model_type], model_type=model_type, alpha=0.7)
+        ref = L['merge_lora'][model_type]
         b = mine.merge_lora_into_weight(sd, ckpt[model_type], model_type=model_type, alpha=0.7)
-        assert a.keys() == b.keys()
-        assert all(torch.equal(a[k], b[k]) for k in a)
-        changed = sum(not torch.equal(a[k], sd[k]) for k in a)
-        assert changed == len(ckpt[model_type]) // 2
+        assert sorted(b.keys()) == ref['keys']
+        changed = sorted(k for k in b if not torch.equal(b[k], sd[k]))
+        assert changed == ref['changed'] and len(changed) == len(ckpt[model_type]) // 2
+        for k, (idx, vals) in ref['samples'].items():
+            assert torch.equal(b[k].reshape(-1)[idx], vals), k
     # load_new_concept on the reference's kind of objects (transformers CLIPTextModel + tokenizer stand-in)
     from transformers import CLIPTextConfig, CLIPTextModel
-    outs = []
-    for fn in (ref.load_new_concept, mine.load_new_concept):
-        torch.manual_seed(0)
-        m = CLIPTextModel(CLIPTextConfig(vocab_size=300, hidden_size=768, intermediate_size=3072, num_hidden_layers=1,
-                                         num_attention_heads=12, max_position_embeddings=77))
-        pipe = SimpleNamespace(tokenizer=FakeTokenizer(300), text_encoder=m)
-        pipe, cfg = fn(pipe, ckpt['new_concept_embedding'], True)
-        outs.append((cfg, m.get_input_embeddings().weight.data[300:].clone()))
-    assert outs[0][0] == outs[1][0] and torch.equal(outs[0][1], outs[1][1])
+    torch.manual_seed(0)
+    m = CLIPTextModel(CLIPTextConfig(vocab_size=300, hidden_size=768, intermediate_size=3072, num_hidden_layers=1,
+                                     num_attention_heads=12, max_position_embeddings=77))
+    pipe = SimpleNamespace(tokenizer=FakeTokenizer(300), text_encoder=m)
+    pipe, cfg = mine.load_new_concept(pipe, ckpt['new_concept_embedding'], True)
+    assert cfg == L['load_new_concept']['cfg']
+    assert torch.equal(m.get_input_embeddings().weight.data[300:], L['load_new_concept']['rows'])

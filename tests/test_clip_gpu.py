@@ -1,4 +1,4 @@
-"""CLIP text encoder on B200 (SURVEY.md 8f rank 1) vs the library the reference itself calls: transformers
+"""CLIP text encoder on the GPU (SURVEY.md 8f rank 1) vs the library the reference itself calls: transformers
 `CLIPTextModel` (random-init from `CLIPTextConfig` with the SD1.5 sizes; fp32 on CPU).  Tolerances: bf16 weights and
 activations through 12 pre-LN layers: rel-L2 <= 2e-2 on the final hidden state (the UNet path measures 8e-3 .. 1e-2)."""
 import pytest
@@ -95,9 +95,9 @@ def test_clip_container_unpadded_ids(cuda):
     """gradient_fusion.py:190-199 calls the text encoder with UN-padded prompts, one at a time: the container pads to the
     engine's fixed length (the encoder is causal) and returns the first L positions - equal to transformers on the same
     ids, and to the prefix of the padded call."""
-    from mixofshow.models.clip_b200 import CLIPTextModel as B200Clip
+    from mixofshow.models.clip_b200 import CLIPTextModel as GpuClip
     model = _clip(2)
-    enc = B200Clip({k: v.clone() for k, v in model.state_dict().items()})
+    enc = GpuClip({k: v.clone() for k, v in model.state_dict().items()})
     ids = torch.tensor([[49406, 320, 1125, 539, 320, 49408 % 49407, 49407]])      # BOS, 5 words, EOS: L = 7
     with torch.no_grad():
         ref = model(ids)[0]

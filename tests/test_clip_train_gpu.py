@@ -1,4 +1,4 @@
-"""Text-encoder half of the ED-LoRA training step on B200 (`mos_b200/clip_train_engine.py`) against fp32 autograd through
+"""Text-encoder half of the ED-LoRA training step on the GPU (`mos_b200/clip_train_engine.py`) against fp32 autograd through
 the library the reference itself calls (transformers `CLIPTextModel`, random-init at the SD1.5 sizes, with the reference's
 LoRA formula y = orig(x) + alpha * up(down(x)) injected, edlora.py:244-246): gradients of the NEW-CONCEPT EMBEDDING ROWS
 (trainer_edlora.py:86-88, train_edlora.py:133-136) and of the 48 CLIPAttention LoRA pairs (:107-118).
@@ -62,7 +62,7 @@ def test_clip_train_engine_vs_transformers_autograd(cuda, layers, n_seq):
     out_ref = model(ids)[0]
     (out_ref * dy).sum().backward()
     g_emb_ref = emb.grad[concept_ids]
-    # ---- B200 engine
+    # ---- GPU engine
     eng = CLIPTrainEngine(sd, n_seq, lora=lora, lora_alpha=alpha, concept_token_ids=concept_ids)
     y = eng.forward_train(ids)
     e_fwd = rel_l2(y.view(n_seq, 77, 768), out_ref.detach())

@@ -1,7 +1,7 @@
-"""Drop-in surface on the GPU: the B200 `mixofshow` package, driven exactly like the reference drives its own modules,
+"""Drop-in surface on the GPU: the GPU `mixofshow` package, driven exactly like the reference drives its own modules,
 against the golden vectors produced by the reference's modules (tests/golden/reference_golden.pt).
 
-Tolerances: golden = fp32 reference; B200 path = bf16 operands / fp32 accumulation -> rel-L2 <= 1.5e-2 on layer
+Tolerances: golden = fp32 reference; GPU path = bf16 operands / fp32 accumulation -> rel-L2 <= 1.5e-2 on layer
 outputs (two chained bf16 GEMMs + attention), <= 2e-2 on a whole UNet; integer quantities bit exact.
 """
 import os
@@ -126,7 +126,7 @@ def _tiny_b200_unet(seed=0):
 
 
 def test_b200_unet_driven_like_the_reference_trainer(cuda, G):
-    """The reference's own recipe (trainer_edlora.py:121-133 + pipeline_edlora.py:93) on the B200 UNet container:
+    """The reference's own recipe (trainer_edlora.py:121-133 + pipeline_edlora.py:93) on the GPU UNet container:
     install processors, inject LoRALinearLayer on every Linear under every `Attention`, call unet(...).sample."""
     from mixofshow.models.edlora import LoRALinearLayer, revise_edlora_unet_attention_forward
     from oracle import inject
@@ -147,7 +147,7 @@ def test_b200_unet_driven_like_the_reference_trainer(cuda, G):
     assert len(keep) == g['n_lora']
     out = unet(g['latents'].cuda(), torch.tensor([g['t'], g['t']]).cuda(), g['ehs'].cuda()).sample
     e = rel_l2(out, g['out'])
-    print(f'B200 UNet (reference recipe) vs reference golden: rel-L2 {e:.3e}')
+    print(f'GPU UNet (reference recipe) vs reference golden: rel-L2 {e:.3e}')
     assert e < 2e-2
     # a LoRA update (an optimiser step in training) must be picked up by the next call
     with torch.no_grad():
@@ -172,7 +172,7 @@ def test_b200_unet_regional_with_adapters(cuda, G, tag):
     out = unet(g['latents'].cuda(), t, g['ehs'].cuda(), cross_attention_kwargs=kw,
                down_block_additional_residuals=[a.clone() for a in ad]).sample
     e = rel_l2(out, g['out'][tag])
-    print(f'regional B200 UNet [{tag}] vs reference golden: rel-L2 {e:.3e}')
+    print(f'regional GPU UNet [{tag}] vs reference golden: rel-L2 {e:.3e}')
     assert e < 2e-2
     out2 = unet(g['latents'].cuda(), t, g['ehs'].cuda(), cross_attention_kwargs=kw,
                 down_block_additional_residuals=[a.clone() for a in ad]).sample      # captured-graph replay

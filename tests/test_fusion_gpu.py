@@ -219,7 +219,7 @@ def test_spatial_fusion_two_concepts_tiny(cuda):
     r0 = (X @ W0.t() - V).norm().item()
     r_or = (X @ W_or.t() - V).norm().item()
     r_new = (X @ Wn.t() - V).norm().item()
-    print(f'spatial fusion {name}: residual W0 {r0:.4e} oracle {r_or:.4e} B200 {r_new:.4e}; '
+    print(f'spatial fusion {name}: residual W0 {r0:.4e} oracle {r_or:.4e} GPU {r_new:.4e}; '
           f'rel Frobenius vs oracle {rel(Wn, W_or):.3e}')
     assert r_new < 0.8 * r0                   # the fused weight explains both concepts better than W0
     assert r_new < 1.10 * r_or                # as well as the fp32 oracle solve (features are bf16 on the GPU)
@@ -228,7 +228,7 @@ def test_spatial_fusion_two_concepts_tiny(cuda):
 
 def test_text_encoder_fusion_two_concepts(cuda):
     """merge_text_encoder (gradient_fusion.py:460-565) on a 2-layer CLIP with two synthetic CLIPAttention LoRAs: the
-    features come from the B200 CLIP engine on sequences padded to 77 (valid rows only), the oracle records them with
+    features come from the GPU CLIP engine on sequences padded to 77 (valid rows only), the oracle records them with
     forward hooks on transformers' CLIPTextModel run on the UN-padded sequences with the merged weights (as the reference
     does) and solves with the reference-style L-BFGS in fp32."""
     from transformers import CLIPTextConfig, CLIPTextModel
@@ -277,9 +277,9 @@ def test_text_encoder_fusion_two_concepts(cuda):
         r0 = (X @ W0.t() - V).norm().item()
         r_or = (X @ W_or.t() - V).norm().item()
         r_new = (X @ Wn.t() - V).norm().item()
-        print(f'text-encoder fusion {name}: residual W0 {r0:.4e} oracle {r_or:.4e} B200 {r_new:.4e}; '
+        print(f'text-encoder fusion {name}: residual W0 {r0:.4e} oracle {r_or:.4e} GPU {r_new:.4e}; '
               f'rel Frobenius vs oracle {rel(Wn, W_or):.3e}')
-        # 44 rows against 768 unknowns per output: the oracle residual is ~0, so the B200 residual (bf16 features,
+        # 44 rows against 768 unknowns per output: the oracle residual is ~0, so the GPU residual (bf16 features,
         # evaluated on the oracle's fp32 features) is bounded relative to the starting point instead
         assert r_new < 0.1 * r0
         assert rel(Wn, W_or) < 2e-2

@@ -92,7 +92,7 @@ def test_compose_concepts_wiring(tmp_path, monkeypatch):
     assert all('attn2.to_k' in k or 'attn2.to_v' in k for k in parsed[2][0])
     assert not any('attn2.to_k' in k or 'attn2.to_v' in k for k in parsed[3][0])
     assert len(parsed[2][0]) + len(parsed[3][0]) == len(torch.load(cfgs[0]['lora_path'])['params']['unet'])
-    # ---- stage recorders; the text encoder runs on CPU through transformers (same call shape as the B200 container)
+    # ---- stage recorders; the text encoder runs on CPU through transformers (same call shape as the GPU container)
     seen = {}
     monkeypatch.setattr(model_io, 'load_text_encoder',
                         lambda path, subfolder='text_encoder', **kw: CLIPTextModel.from_pretrained(os.path.join(path, subfolder)).eval())

@@ -1,4 +1,4 @@
-"""K1/K4 parity: tcgen05 GEMM / implicit-GEMM conv vs a plain PyTorch fp32 reference of the same op.
+"""K1/K4 parity: wgmma GEMM / implicit-GEMM conv vs a plain PyTorch fp32 reference of the same op.
 
 Tolerance: inputs are bf16-exact in both paths, accumulation is fp32 in both, so the only differences are
 summation order and the final bf16 rounding of the output: rel-L2 <= 4e-3 (bf16 eps = 3.9e-3), typically ~2e-3.
@@ -164,7 +164,7 @@ def test_conv3x3_splitk(cuda, splits):
 @pytest.mark.parametrize('case', [dict(conv=(2, 8, 8, 1280), N=1280, splits=15), dict(conv=(2, 16, 16, 1280), N=1280, splits=4),
                                   dict(conv=(2, 12, 24, 320), N=320, splits=3), dict(M=512, K=2560, N=1280, splits=4),
                                   dict(M=200, K=1280, N=640, splits=5), dict(conv=(2, 32, 32, 640), N=640, splits=2),
-                                  dict(conv=(2, 32, 32, 640), N=640, splits=4)])    # last: 256 work items > 148 CTAs
+                                  dict(conv=(2, 32, 32, 640), N=640, splits=4)])    # last: 256 work items > 132 CTAs
 @pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float16])
 def test_splitk_in_kernel_finalize(cuda, case, dtype):
     """mos_gemm_args.tile_counters: the `splits` CTAs of every output tile reduce the partials themselves.  Same summation
@@ -212,9 +212,8 @@ def test_gemm_bad_args(cuda):
 
 
 # ---------------------------------------------------------------------------------------------- fp16 operands
-# Sampling runs the GEMMs on fp16 operands (weights AND activations, mos_b200/engine.py).  tcgen05 kind::f16 takes ONE
-# operand format per MMA: an fp16 x bf16 descriptor faults with "illegal instruction" on B200 (measured in round 2), so the
-# C ABI rejects mixed operand types up front.  Tolerance: operands are exact in both paths, fp32 accumulation, final fp16
+# Sampling runs the GEMMs on fp16 operands (weights AND activations, mos_b200/engine.py).  wgmma takes ONE operand
+# type for A and B, so the C ABI rejects mixed operand types up front.  Tolerance: operands are exact in both paths, fp32 accumulation, final fp16
 # rounding (eps 4.9e-4): rel-L2 <= 6e-4.
 def test_gemm_f16(cuda):
     from mos_b200 import ops

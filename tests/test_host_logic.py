@@ -1,4 +1,5 @@
 """Host-side logic that needs no GPU: weight packing, concat-slot bookkeeping, schedule coefficients, ordering."""
+import json
 import math
 
 import numpy as np
@@ -206,9 +207,9 @@ def test_latent_dataset_and_yml_options(tmp_path):
         assert b0['images'].shape == (2, 4, 2, 2) and len(b0['prompts']) == 2 and b0['masks'].shape == (2, 1, 2, 2)
         seen += [int(x[0, 0, 0]) // 16 for x in list(b0['images']) + list(b1['images'])]
     assert len(seen) == 28 and max(seen.count(i) for i in range(6)) <= 5
-    ref_yml = '/root/reference/options/train/EDLoRA/real/8101_EDLoRA_potter_Cmix_B4_Repeat500.yml'
-    if os.path.exists(ref_yml):
-        opt = yaml.safe_load(open(ref_yml))
-        assert opt['models']['finetune_cfg']['text_embedding']['lr'] == 1e-3 and opt['train']['emb_norm_threshold'] == 0.55
-        params = inspect.signature(EDLoRATrainer.__init__).parameters
-        assert all(k in params for k in opt['models']), 'EDLoRATrainer(**opt["models"]) must accept every key of the yml'
+    # the reference's own training options (8101_EDLoRA_potter_Cmix_B4_Repeat500.yml), stored under tests/golden
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'edlora_train_options.json')) as f:
+        opt = json.load(f)
+    assert opt['models']['finetune_cfg']['text_embedding']['lr'] == 1e-3 and opt['train']['emb_norm_threshold'] == 0.55
+    params = inspect.signature(EDLoRATrainer.__init__).parameters
+    assert all(k in params for k in opt['models']), 'EDLoRATrainer(**opt["models"]) must accept every key of the yml'

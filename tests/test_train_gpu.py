@@ -1,4 +1,4 @@
-"""One ED-LoRA training step (forward, loss incl. attention regulariser, backward, AdamW) on the B200 engine vs the
+"""One ED-LoRA training step (forward, loss incl. attention regulariser, backward, AdamW) on the GPU engine vs the
 fp32 oracle differentiated by torch.autograd (oracle/unet.py + oracle/train_ref.py, the latter pinned against the
 reference's cal_attn_reg golden).
 

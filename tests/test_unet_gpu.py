@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 UNet engine against the fp32 CPU oracle (oracle/unet.py + oracle/inject.py).
+"""End-to-end parity of the GPU UNet engine against the fp32 CPU oracle (oracle/unet.py + oracle/inject.py).
 
 Metric: rel-L2 = ||a-b||_2 / ||b||_2.  The sampling engine runs fp16 operands (weights and activations; fp32 accumulation,
 fp32 statistics) - the reference's own sampling precision - the oracle is fp32.  Tolerances: eps (UNet output) rel-L2 <=

@@ -1,4 +1,4 @@
-"""VAE encoder / decoder on B200 (`mos_b200/vae_engine.py`, SURVEY.md 8f rank 2) against the fp32 oracle restatement of
+"""VAE encoder / decoder on the GPU (`mos_b200/vae_engine.py`, SURVEY.md 8f rank 2) against the fp32 oracle restatement of
 diffusers' AutoencoderKL (oracle/vae.py; "parity unpinned": diffusers is absent and the reference has no vectors for this
 boundary).  Reference call sites: `vae.encode(images).latent_dist.sample() * 0.18215` (trainer_edlora.py:203-204) and
 `vae.decode(latents / 0.18215).sample` (pipeline_edlora.py:303-313).
@@ -77,7 +77,7 @@ def test_vae_container_call_shapes(cuda, tmp_path):
 
 def test_pipeline_decodes_to_pil(cuda):
     """EDLoRAPipeline.__call__ with output_type='pil' (the reference default, pipeline_edlora.py:303-313): latents / 0.18215
-    -> B200 VAE decode -> [0,1] clamp -> PIL, so that `.images[0].save(...)` works as in the reference's scripts."""
+    -> GPU VAE decode -> [0,1] clamp -> PIL, so that `.images[0].save(...)` works as in the reference's scripts."""
     from mixofshow.models.unet_b200 import UNet2DConditionModel
     from mixofshow.models.vae_b200 import AutoencoderKL
     from mixofshow.pipelines.pipeline_edlora import EDLoRAPipeline

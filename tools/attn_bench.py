@@ -43,4 +43,4 @@ for d, nq, nk in [(40, 4096, 4096), (80, 1024, 1024), (160, 256, 256), (160, 64,
     fl = 4.0 * nq * nk * d * B * H
     tiles = B * H * -(-nq // 128) * -(-nk // 128)
     print(f'd={d:3d} nq={nq:5d} nk={nk:5d}: {us:9.1f} us  {fl / us / 1e6:7.1f} TFLOP/s (algorithmic)  '
-          f'{us * 1e-6 * 1.965e9 * 148 / tiles:7.0f} SM-cycles per 128x128 block')
+          f'{us * 1e-6 * 1.98e9 * 132 / tiles:7.0f} SM-cycles per 128x128 block')

@@ -1,4 +1,4 @@
-"""BASELINE config 3 END TO END on one B200: `gradient_fusion.compose_concepts` (the entry point `python gradient_fusion.py`
+"""BASELINE config 3 END TO END on one H100: `gradient_fusion.compose_concepts` (the entry point `python gradient_fusion.py`
 drives) on a synthetic SD1.5-size model directory and 5 synthetic ED-LoRA concept checkpoints in the reference's
 on-disk layout - load, token / embedding merge, text-encoder merge (48 CLIPAttention linears x 500 L-BFGS iterations),
 cross-attention K/V merge (32 x 500), spatial-attention merge (96 x 50, incl. the recorded UNet forwards), save and
@@ -76,7 +76,7 @@ def main():
     from transformers import CLIPTextConfig, CLIPTextModel
     work = tempfile.mkdtemp(prefix='compose_bench_')
     out = {'config': f'gradient_fusion.compose_concepts, {a.concepts} synthetic ED-LoRAs, '
-                     f'{"tiny" if a.tiny else "SD1.5-size"} UNet + 12-layer CLIP text encoder, 1xB200',
+                     f'{"tiny" if a.tiny else "SD1.5-size"} UNet + 12-layer CLIP text encoder, 1xH100',
            'textenc_iters': a.textenc_iters, 'unet_iters': a.unet_iters}
     try:
         t0 = time.perf_counter()

@@ -1,4 +1,4 @@
-"""Wall-clock numbers for BASELINE.json configs 3 and 4 at full size on one B200 (synthetic data, SURVEY.md 8d).
+"""Wall-clock numbers for BASELINE.json configs 3 and 4 at full size on one H100 (synthetic data, SURVEY.md 8d).
 
   python tools/config_bench.py regional      # config 4: 768x1536, 3 regions + 4 adapter maps, 30 DPM-Solver++ steps, CFG 7.5
   python tools/config_bench.py fusion        # config 3: UNet half of gradient fusion, 5 synthetic ED-LoRAs, 500 / 50 iters
@@ -60,7 +60,7 @@ def regional(steps=30):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
     assert torch.isfinite(latents).all()
-    print(json.dumps({'config': 'regionally_controlable_sampling 3-region 768x1536, 30 DPMSolver steps, 1xB200',
+    print(json.dumps({'config': 'regionally_controlable_sampling 3-region 768x1536, 30 DPMSolver steps, 1xH100',
                       'seconds_per_image_unet_loop': round(ms / 1e3, 4), 'ms_per_step': round(ms / steps, 3),
                       'steps_per_s': round(steps / ms * 1e3, 2), 'launches_per_step': eng.launches,
                       'algorithmic_tflop_per_step': 11.11, 'tflops': round(11.11 * steps / ms * 1e3, 1),
@@ -74,7 +74,7 @@ def fusion():
     spatial = [{k: v for k, v in l.items() if 'attn2.to_k' not in k and 'attn2.to_v' not in k} for l in loras]
     crosskv = [{k: v for k, v in l.items() if 'attn2.to_k' in k or 'attn2.to_v' in k} for l in loras]
     alphas = [1.0] * 5
-    out = {'config': 'gradient_fusion merge of 5 ED-LoRAs into SD1.5-topology UNet weights on 1xB200 (UNet half)',
+    out = {'config': 'gradient_fusion merge of 5 ED-LoRAs into SD1.5-topology UNet weights on 1xH100 (UNet half)',
            'workers': gf.FUSION_WORKERS, 'native_driver': gf.FUSION_NATIVE}
     solve_s = []
     _solve_all = gf.solve_all

@@ -8,7 +8,7 @@ of the flat gradient buffer, fused AdamW with grad_scale 1/world.  Checked:
   (2) they equal - to fp32 summation-order tolerance - a single-GPU run that accumulates the same `world` shards into one
       gradient buffer (forward_backward(accumulate=True)) and applies the same optimiser step (the reference's
       gradient-accumulation equivalence, train_edlora.py:73-75,120-130).
-Prints one JSON line on rank 0 (committed under profiles/)."""
+Prints one JSON line on rank 0."""
 import json
 import os
 import sys

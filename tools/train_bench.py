@@ -1,4 +1,4 @@
-"""Training-step throughput of the B200 ED-LoRA path (BASELINE configs 2 and 5): SD1.5 topology, 64x64 latents,
+"""Training-step throughput of the H100 ED-LoRA path (BASELINE configs 2 and 5): SD1.5 topology, 64x64 latents,
 synthetic data, random-init weights.  One process per GPU; the batch is sharded (weak scaling: --batch per GPU) and the
 ONLY collective is one NCCL all-reduce of the flat LoRA gradient (3.19 MB) per step.
 

@@ -31,7 +31,7 @@ masks = masks.cuda()
 pos = [[4, 5]] * B
 
 FAMILIES = {
-    'gemm (fwd+bwd tcgen05 GEMM/conv)': ['gemm'],
+    'gemm (fwd+bwd wgmma GEMM/conv)': ['gemm'],
     'splitk_finalize': ['splitk_finalize'],
     'attention fwd': ['attention_train'],
     'attention bwd (+delta)': ['attention_bwd', 'attn_delta'],
