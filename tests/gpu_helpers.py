@@ -1,0 +1,69 @@
+"""Helpers shared by the kernel parity tests: seeded inputs, the rel-L2 metric, head packing and canary buffers.
+
+A canary buffer is an output allocation larger than the kernel's logical output window, filled with a sentinel bit pattern
+(a NaN in bf16, fp16 and fp32).  After the launch everything outside the window must still hold the sentinel.
+"""
+import torch
+
+SENTINEL = {2: 0x7FA5, 4: 0x7FA5A5A5}          # element size -> bit pattern
+_INT = {2: torch.int16, 4: torch.int32}
+
+
+def rel_l2(a, b):
+    a, b = a.float(), b.float()
+    return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
+
+
+def mk(shape, dev, scale=1.0, seed=0, dtype=torch.bfloat16):
+    g = torch.Generator(device='cpu').manual_seed(seed)
+    return (torch.randn(shape, generator=g) * scale).to(dev).to(dtype)
+
+
+def bits(t):
+    """the raw bits of a 16- or 32-bit tensor (for bitwise comparisons that also hold for NaN patterns)"""
+    return t.view(_INT[t.element_size()])
+
+
+def same_bits(a, b):
+    return torch.equal(bits(a), bits(b))
+
+
+def canary(shape, dev, dtype):
+    t = torch.empty(shape, device=dev, dtype=dtype)
+    bits(t).fill_(SENTINEL[t.element_size()])
+    return t
+
+
+def untouched(buf, window):
+    """True if every element of `buf` outside the boolean mask `window` still holds the sentinel"""
+    return bool((bits(buf)[~window] == SENTINEL[buf.element_size()]).all())
+
+
+def window_mask(buf, *index):
+    m = torch.zeros(buf.shape, dtype=torch.bool, device=buf.device)
+    m[index] = True
+    return m
+
+
+def num_sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def rup(x, m):
+    return (x + m - 1) // m * m
+
+
+def pack_rows(t, dp):
+    """[B, H, n, d] -> the zero-padded head-split row layout [B*H, n, dp]"""
+    B, H, n, d = t.shape
+    out = torch.zeros(B * H, n, dp, device=t.device, dtype=t.dtype)
+    out[..., :d] = t.reshape(B * H, n, d)
+    return out
+
+
+def pack_vt(v, dv):
+    """[B, H, nk, d] -> the zero-padded transposed layout [B*H, dv, nk rounded up to 8]"""
+    B, H, nk, d = v.shape
+    out = torch.zeros(B * H, dv, rup(nk, 8), device=v.device, dtype=v.dtype)
+    out[:, :d, :nk] = v.reshape(B * H, nk, d).transpose(1, 2)
+    return out
