@@ -114,8 +114,9 @@ int mos_attention_fwd(const void* Q, const void* K, const void* Vt, void* out, i
                       float scale, int32_t act_dtype, void* stream);
 
 /* GroupNorm(32)(+SiLU) over NHWC bf16 rows: x [B, HW, ldx] -> y [B, HW, ldy]; partial = fp32 workspace of
- * partial_capacity_floats floats (>= B * 592 * 64 is always enough). The LAST 64 words of the workspace hold the grid-barrier
- * state of the single-launch path and must be zero-initialised once by the caller (never touched afterwards). diffusers ResnetBlock2D.norm1/norm2,
+ * partial_capacity_floats floats, used only by the two-launch fallback (slabs that do not fit the one-pass cluster kernel):
+ * at least B * 64 floats (one chunk of rows per sample), more lets the fallback split each sample into more chunks, and
+ * B * 592 * 64 is always enough. No initialisation is needed. diffusers ResnetBlock2D.norm1/norm2,
  * Transformer2DModel.norm, conv_norm_out (reached from mixofshow/pipelines/pipeline_edlora.py:277). */
 int mos_groupnorm_fwd(const void* x, int64_t ldx, int32_t B, int32_t HW, int32_t C, const float* gamma,
                       const float* beta, float eps, int32_t silu_act, float* partial,

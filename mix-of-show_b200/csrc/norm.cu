@@ -14,21 +14,33 @@ namespace mos {
 
 constexpr int GN_GROUPS = 32;
 
-// partial[b][chunk][g][2] = (sum, sumsq) over rows [chunk*rows_per_chunk, ...) of batch b
+// The statistics of a (sample, group) are accumulated about a pivot p, the group's first element in the sample's first
+// row: sums of (x - p) and (x - p)^2, then mean = p + S/n and var = Q/n - (S/n)^2.  Raw sums of x and x^2 would lose the
+// variance to cancellation once the group's mean is large against its spread (E[x^2] - mean^2 in fp32).  Every chunk and
+// every CTA of a cluster reads the same pivot, so the partials still add up in a fixed order.
+template <bool F16>
+__device__ __forceinline__ float gn_pivot(const __nv_bfloat16* x, long long ldx, int b, int HW, int c0) {
+  return ld16<F16>(x + (long long)b * HW * ldx + c0);
+}
+
+// partial[b][chunk][g][2] = (sum, sumsq) of (x - pivot_g) over rows [chunk*rows_per_chunk, ...) of batch b
 template <bool F16>
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int C,
                                 int rows_per_chunk, float* __restrict__ partial) {
   extern __shared__ float red[];  // [blockDim][16]: per-thread channel sums / sums of squares
   pdl_wait();
   pdl_launch_dependents();
-  const int oct = C / 8;
+  const int oct = C / 8, cpg = C / GN_GROUPS;
   const int b = blockIdx.y, chunk = blockIdx.x, nchunks = gridDim.x;
   const int lanes = blockDim.x / oct;  // row lanes; blockDim is a multiple of oct
   const int o = threadIdx.x % oct, rl = threadIdx.x / oct;
   const int r0 = chunk * rows_per_chunk, r1 = min(HW, r0 + rows_per_chunk);
-  float s[8], q[8];
+  float s[8], q[8], p[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    s[i] = q[i] = 0.f;
+    p[i] = gn_pivot<F16>(x, ldx, b, HW, (o * 8 + i) / cpg * cpg);
+  }
   const __nv_bfloat16* base = x + ((long long)b * HW) * ldx + o * 8;
   for (int rb = r0 + rl; rb < r1; rb += 4 * lanes) {
     uint4 u4[4];   // four independent 16-byte loads in flight per thread
@@ -39,14 +51,16 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long l
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
+      if (rb + k * lanes >= r1) continue;
       const uint32_t w[4] = {u4[k].x, u4[k].y, u4[k].z, u4[k].w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        float2 f = unpack16x2<F16>(w[i]);
-        s[2 * i] += f.x;
-        q[2 * i] += f.x * f.x;
-        s[2 * i + 1] += f.y;
-        q[2 * i + 1] += f.y * f.y;
+        const float2 f = unpack16x2<F16>(w[i]);
+        const float d0 = f.x - p[2 * i], d1 = f.y - p[2 * i + 1];
+        s[2 * i] += d0;
+        q[2 * i] += d0 * d0;
+        s[2 * i + 1] += d1;
+        q[2 * i + 1] += d1 * d1;
       }
     }
   }
@@ -57,7 +71,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long l
   }
   __syncthreads();
   if (threadIdx.x < GN_GROUPS) {  // fixed summation order -> bitwise reproducible statistics
-    const int g = threadIdx.x, cpg = C / GN_GROUPS;
+    const int g = threadIdx.x;
     float gs = 0.f, gq = 0.f;
     for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
       for (int l = 0; l < lanes; ++l) {
@@ -98,10 +112,9 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
     }
     if (sub == 0) {
       const float n = (float)HW * (float)cpg;
-      const float m = s / n;
-      const float var = fmaxf(q / n - m * m, 0.f);
-      mean[g] = m;
-      rstd[g] = rsqrtf(var + eps);
+      const float d = s / n;    // mean - pivot
+      mean[g] = gn_pivot<F16>(x, ldx, b, HW, g * cpg) + d;
+      rstd[g] = rsqrtf(fmaxf(q / n - d * d, 0.f) + eps);
     }
   }
   __syncthreads();
@@ -109,13 +122,14 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
   const int lanes = blockDim.x / oct;
   const int o = threadIdx.x % oct, rl = threadIdx.x / oct;
   if (rl >= lanes) return;
-  float sc[8], sh[8];
+  // y = (x - mean) * (gamma * rstd) + beta: folding the mean into the shift would cancel when |mean| * rstd is large
+  float sc[8], mu[8], sh[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     int c = o * 8 + i, g = c / cpg;
-    float ga = __ldg(gamma + c) * rstd[g];
-    sc[i] = ga;
-    sh[i] = __ldg(beta + c) - mean[g] * ga;
+    sc[i] = __ldg(gamma + c) * rstd[g];
+    mu[i] = mean[g];
+    sh[i] = __ldg(beta + c);
   }
   const int r0 = blockIdx.x * rows_per_block, r1 = min(HW, r0 + rows_per_block);
   const __nv_bfloat16* xb = x + ((long long)b * HW) * ldx + o * 8;
@@ -136,8 +150,8 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           float2 f = unpack16x2<F16>(w[i]);
-          v[2 * i] = f.x * sc[2 * i] + sh[2 * i];
-          v[2 * i + 1] = f.y * sc[2 * i + 1] + sh[2 * i + 1];
+          v[2 * i] = (f.x - mu[2 * i]) * sc[2 * i] + sh[2 * i];
+          v[2 * i + 1] = (f.y - mu[2 * i + 1]) * sc[2 * i + 1] + sh[2 * i + 1];
         }
         if (silu_act) {
 #pragma unroll
@@ -271,6 +285,7 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
   using word_t = typename std::conditional<VEC == 4, uint2, uint32_t>::type;
   word_t* slab = reinterpret_cast<word_t*>(gsm);
   const __nv_bfloat16* xb = x + ((long long)b * HW) * ldx + g * cpg + v * VEC;
+  const float p = gn_pivot<F16>(x, ldx, b, HW, g * cpg);   // sums of x - p and (x - p)^2, see gn_pivot
   float s = 0.f, q = 0.f;
   if (rl < lanes) {
     for (int r = r0 + rl; r < r1; r += 4 * lanes) {
@@ -285,15 +300,17 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
         const int rr = r + j * lanes;
         if (rr < r1) {
           slab[(rr - r0) * vpr + v] = w[j];
-          float2 f0, f1 = make_float2(0.f, 0.f);
           if constexpr (VEC == 4) {
-            f0 = unpack16x2<F16>(w[j].x);
-            f1 = unpack16x2<F16>(w[j].y);
+            const float2 f0 = unpack16x2<F16>(w[j].x), f1 = unpack16x2<F16>(w[j].y);
+            const float d0 = f0.x - p, d1 = f0.y - p, d2 = f1.x - p, d3 = f1.y - p;
+            s += (d0 + d1) + (d2 + d3);
+            q += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
           } else {
-            f0 = unpack16x2<F16>(w[j]);
+            const float2 f0 = unpack16x2<F16>(w[j]);
+            const float d0 = f0.x - p, d1 = f0.y - p;
+            s += d0 + d1;
+            q += d0 * d0 + d1 * d1;
           }
-          s += (f0.x + f0.y) + (f1.x + f1.y);
-          q += (f0.x * f0.x + f0.y * f0.y) + (f1.x * f1.x + f1.y * f1.y);
         }
       }
     }
@@ -332,20 +349,19 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
       tq += table[i].y;
     }
     const float n = (float)HW * (float)cpg;
-    const float m = ts / n;
-    stat[0] = m;
-    stat[1] = rsqrtf(fmaxf(tq / n - m * m, 0.f) + eps);
+    const float d = ts / n;    // mean - pivot
+    stat[0] = p + d;
+    stat[1] = rsqrtf(fmaxf(tq / n - d * d, 0.f) + eps);
   }
   __syncthreads();
   if (rl >= lanes) return;
   const float mean = stat[0], rstd = stat[1];
-  float sc[VEC], sh[VEC];
+  float sc[VEC], sh[VEC];   // y = (x - mean) * sc + sh, as in gn_apply_kernel
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
     const int c = g * cpg + v * VEC + i;
-    const float ga = __ldg(gamma + c) * rstd;
-    sc[i] = ga;
-    sh[i] = __ldg(beta + c) - mean * ga;
+    sc[i] = __ldg(gamma + c) * rstd;
+    sh[i] = __ldg(beta + c);
   }
   __nv_bfloat16* yb = y + ((long long)b * HW) * ldy + g * cpg + v * VEC;
   for (int r = r0 + rl; r < r1; r += lanes) {
@@ -353,14 +369,14 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
     float o[VEC];
     if constexpr (VEC == 4) {
       const float2 f0 = unpack16x2<F16>(w.x), f1 = unpack16x2<F16>(w.y);
-      o[0] = f0.x * sc[0] + sh[0];
-      o[1] = f0.y * sc[1] + sh[1];
-      o[2] = f1.x * sc[2] + sh[2];
-      o[3] = f1.y * sc[3] + sh[3];
+      o[0] = (f0.x - mean) * sc[0] + sh[0];
+      o[1] = (f0.y - mean) * sc[1] + sh[1];
+      o[2] = (f1.x - mean) * sc[2] + sh[2];
+      o[3] = (f1.y - mean) * sc[3] + sh[3];
     } else {
       const float2 f0 = unpack16x2<F16>(w);
-      o[0] = f0.x * sc[0] + sh[0];
-      o[1] = f0.y * sc[1] + sh[1];
+      o[0] = (f0.x - mean) * sc[0] + sh[0];
+      o[1] = (f0.y - mean) * sc[1] + sh[1];
     }
     if (silu_act) {
 #pragma unroll
@@ -387,7 +403,9 @@ __device__ __forceinline__ float silu_grad(float z) {
   return sg * (1.0f + z * (1.0f - sg));
 }
 
-__device__ __forceinline__ void gn_load_stats(const float* __restrict__ partial, int nchunks, int b, int HW, int cpg,
+// mean / rstd of the (sample, group) pairs from the partials of gn_stats_kernel<false> (bf16 x: training)
+__device__ __forceinline__ void gn_load_stats(const __nv_bfloat16* __restrict__ x, long long ldx,
+                                              const float* __restrict__ partial, int nchunks, int b, int HW, int cpg,
                                               float eps, float* mean, float* rstd) {
   if (threadIdx.x < GN_GROUPS * 4) {
     const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
@@ -404,9 +422,9 @@ __device__ __forceinline__ void gn_load_stats(const float* __restrict__ partial,
     }
     if (sub == 0) {
       const float n = (float)HW * (float)cpg;
-      const float m = s / n;
-      mean[g] = m;
-      rstd[g] = rsqrtf(fmaxf(q / n - m * m, 0.f) + eps);
+      const float d = s / n;    // mean - pivot
+      mean[g] = gn_pivot<false>(x, ldx, b, HW, g * cpg) + d;
+      rstd[g] = rsqrtf(fmaxf(q / n - d * d, 0.f) + eps);
     }
   }
 }
@@ -423,7 +441,7 @@ __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, long l
   pdl_launch_dependents();
   const int b = blockIdx.y, chunk = blockIdx.x, nchunks = gridDim.x;
   const int cpg = C / GN_GROUPS;
-  gn_load_stats(partial, nchunks, b, HW, cpg, eps, mean, rstd);
+  gn_load_stats(x, ldx, partial, nchunks, b, HW, cpg, eps, mean, rstd);
   __syncthreads();
   const int oct = C / 8;
   const int lanes = blockDim.x / oct;
@@ -494,7 +512,7 @@ __global__ void gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long lo
   pdl_launch_dependents();
   const int b = blockIdx.y, nchunks = gridDim.x;
   const int cpg = C / GN_GROUPS;
-  gn_load_stats(partial, nchunks, b, HW, cpg, eps, mean, rstd);
+  gn_load_stats(x, ldx, partial, nchunks, b, HW, cpg, eps, mean, rstd);
   if (threadIdx.x < GN_GROUPS * 4) {
     const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
     float s = 0.f, q = 0.f;
@@ -683,8 +701,8 @@ extern "C" int mos_debug_set_gn_twopass(int32_t on) {   // A/B switch for tools/
 }
 
 // GroupNorm(32) + optional SiLU:  y[b, r, c] = act((x - mean_bg) * rstd_bg * gamma_c + beta_c)
-// x: bf16 [B, HW, ldx] (first C channels), y: bf16 [B, HW, ldy]; partial: fp32 workspace [B, nchunks, 32, 2],
-// nchunks = *nchunks_io (0 = choose; the chosen value is returned through the pointer).
+// x: bf16 [B, HW, ldx] (first C channels), y: bf16 [B, HW, ldy]; partial: fp32 workspace [B, nchunks, 32, 2] of the
+// fallback, nchunks chosen to fit partial_capacity_floats (at least B * 64).
 extern "C" int mos_groupnorm_fwd(const void* x, int64_t ldx, int32_t B, int32_t HW, int32_t C, const float* gamma,
                                  const float* beta, float eps, int32_t silu_act, float* partial,
                                  int32_t partial_capacity_floats, void* y, int64_t ldy, int32_t act_dtype,
@@ -760,7 +778,7 @@ extern "C" int mos_groupnorm_fwd(const void* x, int64_t ldx, int32_t B, int32_t 
   int min_rows = 4 * (threads / (C / 8));
   if (nchunks > (int)ceil_div(HW, min_rows)) nchunks = (int)ceil_div(HW, min_rows);
   {
-    const long long cap = ((long long)partial_capacity_floats - 64) / ((long long)B * GN_GROUPS * 2);
+    const long long cap = (long long)partial_capacity_floats / ((long long)B * GN_GROUPS * 2);
     if (nchunks > cap) nchunks = (int)cap;
   }
   if (nchunks < 1) nchunks = 1;

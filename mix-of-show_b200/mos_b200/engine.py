@@ -246,7 +246,7 @@ class UNetEngine:
         self.in_t = torch.zeros(B, device=self.dev)
         self.in_ehs = torch.zeros(len(self.xattn_names), B, self.n_text, self.cross_dim, device=self.dev, dtype=self.ACT)
         self.out_eps = torch.zeros(B, 4, H, W, device=self.dev)
-        self.gn_partial = torch.zeros(B * 592 * 64, device=self.dev)   # tail words: grid-barrier state (zero once)
+        self.gn_partial = torch.zeros(B * 592 * 64, device=self.dev)   # GroupNorm fallback workspace: enough for any HW
         # concat buffers of the 12 up-block resnets: [h | skip]
         nb = len(self.block_out)
         rev = list(reversed(self.block_out))

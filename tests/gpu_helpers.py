@@ -53,6 +53,28 @@ def rup(x, m):
     return (x + m - 1) // m * m
 
 
+def gn_path(B, HW, C, ldx, ldy, sms=None):
+    """The GroupNorm forward implementation `mos_groupnorm_fwd` picks for these arguments (unless the two-pass switch is
+    on): ('cluster', k, vec) for the one-pass kernel with a cluster of k CTAs and vec-element words, or 'fallback' for
+    the statistics + apply launches.  A copy of the host rule in csrc/norm.cu, mos_groupnorm_fwd ("one-pass path" block:
+    the vec choice, the k-widening loop and the 200 KB shared-memory test); keep the two in step."""
+    import os
+    sms = num_sms() if sms is None else sms
+    cpg = C // 32
+    vec = 4 if cpg % 4 == 0 and ldx % 4 == 0 and ldy % 4 == 0 else 2
+    slab = HW * cpg * 2
+    min_ctas = int(os.environ.get('MOS_GN_MIN_CTAS', '0')) or 2 * sms
+    if min_ctas < 1:
+        min_ctas = 2 * sms
+    k = 1
+    while k < 8 and HW // (2 * k) >= 16 and (slab // k > 48 * 1024 or B * 32 * k < min_ctas):
+        k *= 2
+    smem = -(-HW // k) * cpg * 2
+    if smem <= 200 * 1024 and cpg % 2 == 0 and ldx % 2 == 0 and ldy % 2 == 0:
+        return ('cluster', k, vec)
+    return 'fallback'
+
+
 def pack_rows(t, dp):
     """[B, H, n, d] -> the zero-padded head-split row layout [B*H, n, dp]"""
     B, H, n, d = t.shape

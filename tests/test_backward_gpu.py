@@ -22,41 +22,91 @@ def mk(shape, dev, scale=1.0, seed=0):
     return (torch.randn(shape, generator=g) * scale).to(dev).to(BF)
 
 
+def _row_offsets(M, dev, ratio, seed):
+    """a per-row offset of `ratio` x the rows' std (1.5), with a random sign per row"""
+    g = torch.Generator(device='cpu').manual_seed(seed)
+    return (torch.where(torch.rand(M, 1, generator=g) < 0.5, -1.0, 1.0) * 1.5 * ratio).to(dev)
+
+
+def _check_layernorm_bwd(cuda, M, C, ld=None, off=0):
+    """x rows with pitch ld (default C) and a per-row offset of `off` x the rows' std, vs float64 autograd"""
+    from mos_b200 import ops
+    ld = C if ld is None else ld
+    buf = (mk((M, ld), cuda, 1.5, 1).float() + _row_offsets(M, cuda, off, 4)).to(BF)
+    x = buf[:, :C]
+    dy, add = mk((M, C), cuda, 1.0, 2), mk((M, C), cuda, 1.0, 3)
+    gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
+    xr = x.double().requires_grad_(True)
+    F.layer_norm(xr, (C,), gamma.double(), beta.double(), 1e-5).backward(dy.double())
+    dx = torch.empty(M, C, device=cuda, dtype=BF)
+    ops.layernorm_bwd(buf, dy, gamma, dx, M=M, C=C, ldx=ld)
+    assert rel_l2(dx, xr.grad) < 4e-3
+    ops.layernorm_bwd(buf, dy, gamma, dx, M=M, C=C, add=add, ldx=ld)
+    assert rel_l2(dx, xr.grad + add.double()) < 4e-3
+
+
 @pytest.mark.parametrize('M,C', [(8192, 320), (2048, 640), (300, 1280)])
 def test_layernorm_bwd(cuda, M, C):
+    _check_layernorm_bwd(cuda, M, C)
+
+
+# C = 768 with ldx = 800 is the CLIP engines' hidden-state pitch; off: row mean / std
+@pytest.mark.parametrize('off', [0, 100])
+def test_layernorm_bwd_pitched_offset(cuda, off):
+    _check_layernorm_bwd(cuda, 154, 768, ld=800, off=off)
+
+
+# off: group mean / std (a per-(sample, group) offset); pad: extra columns of dy, dx and add (lddy = lddx = ldadd = C + pad);
+# ws: workspace floats (B * 128 holds one chunk of both partial tables)
+def _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off=0, pad=0, ws=1 << 18):
+    from gpu_helpers import canary, untouched, window_mask
     from mos_b200 import ops
-    x, dy, add = mk((M, C), cuda, 1.5, 1), mk((M, C), cuda, 1.0, 2), mk((M, C), cuda, 1.0, 3)
+    g = torch.Generator(device='cpu').manual_seed(5)
+    sign = torch.where(torch.rand(B, 1, 32, 1, generator=g) < 0.5, -1.0, 1.0)
+    shift = (sign * 1.5 * off).expand(B, 1, 32, C // 32).reshape(B, 1, C).to(cuda)
+    buf = mk((B, HW, ld), cuda, 1.5, 1).float() + 0.3
+    buf[..., :C] += shift
+    buf = buf.to(BF)
+    x = buf[..., :C]
+    ldp = C + pad
+    dyb = torch.full((B, HW, ldp), float('nan'), device=cuda, dtype=BF)
+    addb = torch.full((B, HW, ldp), float('nan'), device=cuda, dtype=BF)
+    dyb[..., :C], addb[..., :C] = mk((B, HW, C), cuda, 1.0, 2), mk((B, HW, C), cuda, 1.0, 3)
+    dy, add = dyb[..., :C], addb[..., :C]
     gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
-    xr = x.float().requires_grad_(True)
-    F.layer_norm(xr, (C,), gamma, beta, 1e-5).backward(dy.float())
-    dx = torch.empty_like(x)
-    ops.layernorm_bwd(x, dy, gamma, dx, M=M, C=C)
-    assert rel_l2(dx, xr.grad) < 4e-3
-    ops.layernorm_bwd(x, dy, gamma, dx, M=M, C=C, add=add)
-    assert rel_l2(dx, xr.grad + add.float()) < 4e-3
+    xr = x.double().permute(0, 2, 1).contiguous().requires_grad_(True)       # [B, C, HW]
+    y = F.group_norm(xr, 32, gamma.double(), beta.double(), 1e-5)
+    if silu:
+        y = F.silu(y)
+    y.backward(dy.double().permute(0, 2, 1))
+    ref = xr.grad.permute(0, 2, 1)
+    wsb = torch.empty(ws, device=cuda)
+    dxb = canary((B * HW + 2, ldp), cuda, BF)
+    dx = dxb[:B * HW, :C].view(B, HW, C)
+    ops.groupnorm_bwd(x, dy, gamma, beta, dx, wsb, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld, lddy=ldp, lddx=ldp)
+    assert untouched(dxb, window_mask(dxb, slice(0, B * HW), slice(0, C)))
+    e = rel_l2(dx, ref)
+    ops.groupnorm_bwd(x, dy, gamma, beta, dx, wsb, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld, lddy=ldp, lddx=ldp,
+                      add=add, ldadd=ldp)
+    e_add = rel_l2(dx, ref + add.double())
+    print(f'GN bwd B={B} HW={HW} C={C} offset {off} pad {pad} ws {ws}: rel-L2 {e:.2e}, with add {e_add:.2e}')
+    assert e < 5e-3 and e_add < 5e-3
 
 
 @pytest.mark.parametrize('B,HW,C,ld,silu', [(2, 4096, 320, 320, True), (2, 1024, 1920, 1920, True),
                                              (2, 256, 640, 1280, False), (3, 64, 1280, 1280, True),
                                              (1, 1024, 960, 960, True)])
 def test_groupnorm_bwd(cuda, B, HW, C, ld, silu):
-    from mos_b200 import ops
-    buf = mk((B, HW, ld), cuda, 1.5, 1) + 0.3
-    x = buf[..., :C]
-    dy, add = mk((B, HW, C), cuda, 1.0, 2), mk((B, HW, C), cuda, 1.0, 3)
-    gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
-    xr = x.float().permute(0, 2, 1).contiguous().requires_grad_(True)       # [B, C, HW]
-    y = F.group_norm(xr, 32, gamma, beta, 1e-5)
-    if silu:
-        y = F.silu(y)
-    y.backward(dy.float().permute(0, 2, 1))
-    ref = xr.grad.permute(0, 2, 1)
-    ws = torch.empty(1 << 18, device=cuda)
-    dx = torch.empty(B, HW, C, device=cuda, dtype=BF)
-    ops.groupnorm_bwd(x, dy, gamma, beta, dx, ws, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld)
-    assert rel_l2(dx, ref) < 5e-3
-    ops.groupnorm_bwd(x, dy, gamma, beta, dx, ws, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld, add=add)
-    assert rel_l2(dx, ref + add.float()) < 5e-3
+    _check_groupnorm_bwd(cuda, B, HW, C, ld, silu)
+
+
+@pytest.mark.parametrize('B,HW,C,ld,silu,off,pad,ws', [
+    (2, 4096, 320, 320, True, 10, 32, 1 << 18), (2, 1024, 640, 1280, True, 30, 16, 1 << 18),
+    (1, 1024, 960, 960, True, 100, 40, 1 << 18), (2, 256, 1280, 1280, False, 100, 8, 1 << 18),
+    (2, 4096, 320, 320, True, 100, 0, 2 * 128), (3, 64, 1280, 1280, True, 30, 24, 3 * 128)])
+def test_groupnorm_bwd_offset_pitched(cuda, B, HW, C, ld, silu, off, pad, ws):
+    """group means up to 100 x their std, dy / dx / add pitches above C, and a one-chunk workspace"""
+    _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off, pad, ws)
 
 
 def test_geglu_fwd_bwd(cuda):

@@ -99,7 +99,7 @@ def test_groupnorm(cuda, B, HW, C, ld, silu):
     x = buf[..., :C]
     gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
     y = torch.empty((B, HW, C), device=cuda, dtype=torch.bfloat16)
-    partial = torch.zeros(B * 592 * 64, device=cuda)   # the tail holds the (zero-initialised) grid-barrier state
+    partial = torch.zeros(B * 592 * 64, device=cuda)   # the engines' workspace: enough for any B, HW
     ops.groupnorm(buf, gamma, beta, y, partial, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld)
     ref = F.group_norm(x.float().transpose(1, 2), 32, gamma, beta, 1e-5)
     if silu:
@@ -107,14 +107,30 @@ def test_groupnorm(cuda, B, HW, C, ld, silu):
     assert rel_l2(y, ref.transpose(1, 2)) < 4e-3
 
 
+def _check_layernorm(cuda, M, C, ld=None, off=0):
+    """x rows with pitch ld (default C) and a per-row offset of `off` x the rows' std, vs float64"""
+    from mos_b200 import ops
+    ld = C if ld is None else ld
+    g = torch.Generator(device='cpu').manual_seed(2)
+    shift = (torch.where(torch.rand(M, 1, generator=g) < 0.5, -1.0, 1.0) * 2 * off).to(cuda)
+    buf = (mk((M, ld), cuda, seed=1).float() * 2 + 0.5 + shift).to(torch.bfloat16)
+    x = buf[:, :C]
+    gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
+    y = torch.empty(M, C, device=cuda, dtype=torch.bfloat16)
+    ops.layernorm(buf, gamma, beta, y, M=M, C=C, ldx=ld)
+    ref = F.layer_norm(x.double(), (C,), gamma.double(), beta.double(), 1e-5)
+    assert rel_l2(y, ref) < 4e-3
+
+
 @pytest.mark.parametrize('M,C', [(8192, 320), (2048, 640), (512, 1280), (154, 320)])
 def test_layernorm(cuda, M, C):
-    from mos_b200 import ops
-    x = mk((M, C), cuda, seed=1) * 2 + 0.5
-    gamma, beta = torch.randn(C, device=cuda), torch.randn(C, device=cuda)
-    y = torch.empty_like(x)
-    ops.layernorm(x, gamma, beta, y, M=M, C=C)
-    assert rel_l2(y, F.layer_norm(x.float(), (C,), gamma, beta, 1e-5)) < 4e-3
+    _check_layernorm(cuda, M, C)
+
+
+# C = 768 with ldx = 800 is the CLIP engines' hidden-state pitch; off: row mean / std
+@pytest.mark.parametrize('off', [0, 100])
+def test_layernorm_pitched_offset(cuda, off):
+    _check_layernorm(cuda, 154, 768, ld=800, off=off)
 
 
 def test_time_embedding_and_gemv(cuda):

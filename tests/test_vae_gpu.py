@@ -16,35 +16,55 @@ def rel_l2(a, b):
     return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
 
 
-@pytest.mark.parametrize('cfg_name,B,H,W', [('tiny', 2, 64, 64), ('tiny', 1, 64, 128), ('sd15', 1, 256, 256)])
-def test_vae_encode_decode(cuda, cfg_name, B, H, W):
+def _check_encode_decode(cuda, cfg_name, B, H, W, decode=True):
+    from gpu_helpers import gn_path, rup
     from mos_b200.vae_engine import VAEEngine
     from oracle import vae as ov
     cfg = ov.TINY_VAE if cfg_name == 'tiny' else None
     ref = ov.build_vae(0, cfg)
     full = dict(ov.SD15_VAE, **(cfg or {}))
-    sd = {k: v.detach() for k, v in ref.state_dict().items()}
+    sd = {k: v.detach().clone() for k, v in ref.state_dict().items()}
+    c0 = full['block_out_channels'][0]
+    if H * W >= 512 * 512:
+        assert gn_path(B, H * W, c0, rup(c0, 160), c0) == 'fallback'
+        ref = ref.to(cuda)
+    dev = next(ref.parameters()).device
     eng = VAEEngine(sd, B, H, W, block_out=full['block_out_channels'], layers=full['layers_per_block'])
     g = torch.Generator().manual_seed(1)
     img = torch.rand(B, 3, H, W, generator=g) * 2 - 1
     d = 2 ** (len(full['block_out_channels']) - 1)
     noise = torch.randn(B, 4, H // d, W // d, generator=g)
     with torch.no_grad():
-        mean_ref, logvar_ref = ref.moments(img)
-        lat_ref = ref.encode_sample(img, noise) * 0.18215
+        mean_ref, logvar_ref = ref.moments(img.to(dev))
+        lat_ref = ref.encode_sample(img.to(dev), noise.to(dev)) * 0.18215
     mean, logvar, lat = eng.encode(img.cuda(), noise=noise.cuda())
     torch.cuda.synchronize()
     e_m, e_v, e_l = rel_l2(mean, mean_ref), rel_l2(logvar, logvar_ref), rel_l2(lat, lat_ref)
     n_enc = eng.launches
-    z = torch.randn(B, 4, H // d, W // d, generator=g)
-    with torch.no_grad():
-        dec_ref = ref.decode(z)
-    dec = eng.decode(z.cuda())
-    torch.cuda.synchronize()
-    e_d = rel_l2(dec, dec_ref)
-    print(f'VAE [{cfg_name}] {B}x3x{H}x{W}: mean rel-L2 {e_m:.3e}, logvar {e_v:.3e}, latents {e_l:.3e} ({n_enc} launches); '
-          f'decode rel-L2 {e_d:.3e} ({eng.launches} launches)')
+    msg = f'VAE [{cfg_name}] {B}x3x{H}x{W}: mean rel-L2 {e_m:.3e}, logvar {e_v:.3e}, latents {e_l:.3e} ({n_enc} launches)'
+    e_d = 0.0
+    if decode:
+        z = torch.randn(B, 4, H // d, W // d, generator=g)
+        with torch.no_grad():
+            dec_ref = ref.decode(z.to(dev))
+        dec = eng.decode(z.cuda())
+        torch.cuda.synchronize()
+        e_d = rel_l2(dec, dec_ref)
+        msg += f'; decode rel-L2 {e_d:.3e} ({eng.launches} launches)'
+    print(msg)
     assert max(e_m, e_v, e_l, e_d) < 5e-3
+
+
+@pytest.mark.parametrize('cfg_name,B,H,W', [('tiny', 2, 64, 64), ('tiny', 1, 64, 128), ('sd15', 1, 256, 256)])
+def test_vae_encode_decode(cuda, cfg_name, B, H, W):
+    _check_encode_decode(cuda, cfg_name, B, H, W)
+
+
+# 512 x 512 is the resolution training encodes (B = 2 per GPU, encode only) and the pipeline decodes; it is the only size
+# at which the VAE's full-resolution GroupNorms take the two-launch fallback.  Its fp32 oracle runs on the GPU (TF32 off).
+@pytest.mark.parametrize('B,decode', [(1, True), (2, False)], ids=['B1', 'B2-encode'])
+def test_vae_encode_decode_512(cuda, B, decode):
+    _check_encode_decode(cuda, 'sd15', B, 512, 512, decode)
 
 
 def test_vae_container_call_shapes(cuda, tmp_path):
