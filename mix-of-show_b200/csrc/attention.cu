@@ -65,6 +65,33 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// O += P V over the first NSTEP k16 steps of a KV tile: one straight-line wgmma chain.  pa holds the P fragments, packed
+// before the fence (a register written between wgmma.fence and the wgmma that reads it makes ptxas inject a warpgroup
+// arrive), and the chain length is a compile-time constant (a wgmma under a runtime guard makes ptxas serialise them all).
+template <int NSTEP, int DV, bool F16, int NKK>
+__device__ __forceinline__ void pv_chain(float (&o)[DV / 2], const uint32_t (&pa)[NKK][4], const uint8_t* sV) {
+  wgmma_fence_regs(o);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < NSTEP; ++kk) {
+    const uint64_t vd = make_desc_sw128(smem_u32(sV + (kk >> 2) * (DV * 128))) + 2 * (kk & 3);
+    wgmma_rs<DV, F16>(o, pa[kk], vd, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+}
+// ksteps (1..NSTEP) -> the chain of that length: every KV tile but a partial last one takes the NSTEP = BKV / 16 chain
+template <int NSTEP, int DV, bool F16, int NKK>
+__device__ __forceinline__ void pv_dispatch(int ksteps, float (&o)[DV / 2], const uint32_t (&pa)[NKK][4],
+                                            const uint8_t* sV) {
+  if (ksteps == NSTEP) {
+    pv_chain<NSTEP, DV, F16>(o, pa, sV);
+  } else if constexpr (NSTEP > 1) {
+    pv_dispatch<NSTEP - 1, DV, F16>(ksteps, o, pa, sV);
+  }
+}
+
 template <int D, bool ONE, bool CAUSAL = false, bool F16 = false>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -82,7 +109,9 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
-  const int T = (p.nk + C::BKV - 1) / C::BKV;
+  // ONE: the host launches it only for nk <= 128, so there is one KV tile; as a constant it lets the compiler see that
+  // O is still zero while S is computed, instead of keeping (or spilling) its registers across that wgmma chain
+  const int T = ONE ? 1 : (p.nk + C::BKV - 1) / C::BKV;
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ);
@@ -140,8 +169,10 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     pos1 = __ldg(p.pos + bb * 2 + 1);
   }
   float o[NO];
+  if constexpr (!ONE) {                     // (ONE: O is zeroed right before its one PV chain)
 #pragma unroll
-  for (int i = 0; i < NO; ++i) o[i] = 0.f;
+    for (int i = 0; i < NO; ++i) o[i] = 0.f;
+  }
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, pc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
   mbar_wait(&q_full, 0);
   const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + wg * (64 * 128)));
@@ -188,10 +219,12 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
       l[hr] *= alpha;
       pc[hr][0] *= alpha;
       pc[hr][1] *= alpha;
+      if constexpr (!ONE) {                 // (ONE: O = +0 and alpha = ex2(-inf) = +0, so O * alpha is +0)
 #pragma unroll
-      for (int i = 0; i < C::DV / 8; ++i) {
-        o[4 * i + 2 * hr] *= alpha;
-        o[4 * i + 2 * hr + 1] *= alpha;
+        for (int i = 0; i < C::DV / 8; ++i) {
+          o[4 * i + 2 * hr] *= alpha;
+          o[4 * i + 2 * hr + 1] *= alpha;
+        }
       }
       float rs = 0.f;
 #pragma unroll
@@ -227,20 +260,15 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUt
     }
     // ---- O += P V (P from registers; k-steps past the last valid key are skipped: those columns of V^T may be padding)
     const int ksteps = (kv_valid + 15) >> 4;
-    wgmma_fence_regs(o);
-    wgmma_fence();
+    uint32_t pa[C::BKV / 16][4];
 #pragma unroll
-    for (int kk = 0; kk < C::BKV / 16; ++kk) {
-      if (kk < ksteps) {
-        uint32_t a[4];
-        frag_to_a<F16>(&s[8 * kk], a);
-        const uint64_t vd = make_desc_sw128(smem_u32(sV + (kk >> 2) * (C::DV * 128))) + 2 * (kk & 3);
-        wgmma_rs<C::DV, F16>(o, a, vd, 1u);
-      }
+    for (int kk = 0; kk < C::BKV / 16; ++kk) frag_to_a<F16>(&s[8 * kk], pa[kk]);
+    if constexpr (ONE) {
+#pragma unroll
+      for (int i = 0; i < NO; ++i) o[i] = 0.f;
+      wgmma_fence_regs(o);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(o);
+    pv_dispatch<C::BKV / 16, C::DV, F16>(ksteps, o, pa, sV);
     __syncwarp();
     if (lane == 0) mbar_arrive(&kv_empty[st]);
     if (++st == C::STAGES) {

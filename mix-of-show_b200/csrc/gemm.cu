@@ -37,7 +37,6 @@ struct GemmDev {
   int kb_per_split;
   int stages;
   int conv, H, W, B, kc_per_tap, TW, TH, TB, lgTW, lgTH, tiles_w, tiles_h;
-  int lora;
   int geglu;
   int out_mode;
   int splits;
@@ -121,21 +120,36 @@ __device__ __forceinline__ float col_bias(const GemmDev& p, int b, int n) {
   if (p.bias_batch) v += __ldg(p.bias_batch + (long long)b * p.bias_batch_ld + n);
   return v;
 }
+// LoRA: the rank values t[4 seg .. 4 seg + 3] (segment seg = 0..3) of tile row rA + 8 hr.  The 16 values of a row lie in
+// the LoRA accumulator fragment of the 4 lanes of a quad: t[8h + 2s + e] = lacc[4h + 2hr + e] of quad lane s.  The quad
+// shares its row, so it is either wholly inside the output or wholly outside: the shuffles name only its 4 lanes.  Only
+// compile-time indices into lacc (selects), so that nothing lives in local memory.
+__device__ __forceinline__ float4 lora_ranks(const float (&lacc)[LORA_N / 2], int hr, int seg, int lane) {
+  const unsigned quad = 0xFu << (lane & ~3);
+  const bool hi = seg >= 2;
+  const float v0 = hi ? lacc[4 + 2 * hr] : lacc[2 * hr];
+  const float v1 = hi ? lacc[5 + 2 * hr] : lacc[1 + 2 * hr];
+  const int s = 2 * (seg & 1);
+  return make_float4(__shfl_sync(quad, v0, s, 4), __shfl_sync(quad, v1, s, 4), __shfl_sync(quad, v0, s + 1, 4),
+                     __shfl_sync(quad, v1, s + 1, 4));
+}
 // LoRA term of output column n: t[4 ranks of n's segment] . (alpha * up)[n]
-__device__ __forceinline__ float lora_term(const GemmDev& p, const float* t, int n) {
+__device__ __forceinline__ float lora_term(const GemmDev& p, float4 t, int n) {
   const float4 u = __ldg(reinterpret_cast<const float4*>(p.lora_up) + n);
-  return t[0] * u.x + t[1] * u.y + t[2] * u.z + t[3] * u.w;
+  return t.x * u.x + t.y * u.y + t.z * u.z + t.w * u.w;
 }
 
 // F16: 16-bit type of A, of the row / head-split outputs and of the residual (fp16 or bf16).
-template <bool F16>
+// LORA: the fused LoRA branch is present (a template parameter, so that the k16 wgmma chain of a k block is straight-line
+// code in both variants: a runtime branch between two wgmmas makes ptxas serialise them).
+template <bool F16, bool LORA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmL, const GemmDev p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by SWIZZLE_128B
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int stage_bytes = A_STAGE_BYTES + (p.lora ? BN + LORA_N : BN) * 128;
+  constexpr int stage_bytes = A_STAGE_BYTES + (LORA ? BN + LORA_N : BN) * 128;
 
   __shared__ uint64_t full_bar[MAX_STAGES];
   __shared__ uint64_t empty_bar[MAX_STAGES];
@@ -147,7 +161,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (p.lora) tma_prefetch_desc(&tmL);
+    if (LORA) tma_prefetch_desc(&tmL);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);                          // one arrive.expect_tx by the producer
       mbar_init(&empty_bar[s], CONSUMER_THREADS / 32);     // one arrival per consumer warp
@@ -196,7 +210,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, t.m0);
           }
           tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, t.n0);
-          if (p.lora) tma_load_2d(sb + B_STAGE_BYTES, &tmL, &full_bar[stage], kb * BK, 0);
+          if (LORA) tma_load_2d(sb + B_STAGE_BYTES, &tmL, &full_bar[stage], kb * BK, 0);
           if (++stage == p.stages) {
             stage = 0;
             phase ^= 1;
@@ -223,6 +237,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 #pragma unroll
       for (int i = 0; i < LORA_N / 2; ++i) lacc[i] = 0.f;
+      // One k block stays in flight: k block kb is issued before the wgmmas of kb - 1 are waited for, and only then is
+      // kb - 1's slot handed back to the producer.  The wgmma sequence on the accumulator is the same as with a full
+      // drain per k block, so the result is bit-identical; only the issue overlaps.
+      int prev = -1;                                       // stage of the k block still in flight
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         if (it == 0 && kb == kb_begin && et == 0) stamp(3);
@@ -231,46 +249,43 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const uint64_t bdesc = make_desc_sw128(smem_u32(smem + stage * stage_bytes + A_STAGE_BYTES));
         const uint64_t ldesc = make_desc_sw128(smem_u32(smem + stage * stage_bytes + A_STAGE_BYTES + B_STAGE_BYTES));
         wgmma_fence_regs(acc);
-        wgmma_fence_regs(lacc);
+        if constexpr (LORA) wgmma_fence_regs(lacc);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
           wgmma_ss<BN, F16>(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
-          if (p.lora) wgmma_ss<LORA_N, F16>(lacc, adesc + 2 * k, ldesc + 2 * k, 1u);
+          if constexpr (LORA) wgmma_ss<LORA_N, F16>(lacc, adesc + 2 * k, ldesc + 2 * k, 1u);
         }
         wgmma_commit();
-        wgmma_wait<0>();
+        wgmma_wait<1>();                                   // k block kb - 1 has retired
         wgmma_fence_regs(acc);
-        wgmma_fence_regs(lacc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the slot are done
+        if constexpr (LORA) wgmma_fence_regs(lacc);
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);   // this warp's reads of kb - 1's slot are done
+        }
+        prev = stage;
         if (++stage == p.stages) {
           stage = 0;
           phase ^= 1;
         }
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if constexpr (LORA) wgmma_fence_regs(lacc);
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
       if (et == 0 && it == 0) stamp(4);
       // ---- epilogue, straight from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e)
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        // LoRA: the 16 rank values t of this row are spread over the 4 lanes of a quad; gather them
-        float trow[LORA_N];
-        if (p.lora && p.splits == 1) {
-#pragma unroll
-          for (int s = 0; s < 4; ++s) {
-            const int src = (lane & ~3) | s;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              trow[8 * h + 2 * s] = __shfl_sync(0xffffffffu, lacc[4 * h + 2 * hr], src);
-              trow[8 * h + 2 * s + 1] = __shfl_sync(0xffffffffu, lacc[4 * h + 2 * hr + 1], src);
-            }
-          }
-        }
         const int r = rA + 8 * hr;
         long long m;
         int b;
         if (!row_coord(p, t, r, m, b)) continue;
-        if (p.splits > 1) {
+        if (!LORA && p.splits > 1) {               // (the host rejects LoRA together with split-K)
           float* dst = p.partial + ((long long)t.split * p.M + m) * p.N + t.n0 + cq;
 #pragma unroll
           for (int i = 0; i < BN / 8; ++i)
@@ -278,6 +293,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         } else if (p.geglu) {
           // tile columns [0,80) = a, [80,160) = gate for the same 80 outputs (columns n0/2 + [0,80) of the output)
           __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(p.out) + m * p.ldc + t.n0 / 2;
+          float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f);
+          if constexpr (LORA) t0 = lora_ranks(lacc, hr, 0, lane);
 #pragma unroll
           for (int i = 0; i < BN / 16; ++i) {
             const int na = 8 * i + cq, ng = na + BN / 2;
@@ -286,23 +303,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             for (int e = 0; e < 2; ++e) {
               float a = acc[4 * i + 2 * hr + e] + col_bias(p, b, t.n0 + na + e);
               float g = acc[4 * (i + BN / 16) + 2 * hr + e] + col_bias(p, b, t.n0 + ng + e);
-              if (p.lora) {
-                a += lora_term(p, trow, t.n0 + na + e);
-                g += lora_term(p, trow, t.n0 + ng + e);
+              if constexpr (LORA) {
+                a += lora_term(p, t0, t.n0 + na + e);
+                g += lora_term(p, t0, t.n0 + ng + e);
               }
               o[e] = a * gelu_erf(g);
             }
             *reinterpret_cast<uint32_t*>(orow + na) = pack16x2<F16>(o[0], o[1]);
           }
         } else {
+          int seg = -1;                             // LoRA segment whose rank values are in tt
+          float4 tt = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
           for (int i = 0; i < BN / 8; ++i) {
             const int nc = t.n0 + 8 * i + cq;       // global column of the pair (nc, nc + 1)
             float o[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + col_bias(p, b, nc + e);
-            if (p.lora) {
-              const float* tt = trow + 4 * (int)(nc / p.lora_seg);
+            if constexpr (LORA) {
+              // segments are multiples of 16 columns wide: seg is the same for the whole 8-column group, so uniform
+              // over the warp, and it changes at most 3 times along the tile
+              const int sg = nc / (int)p.lora_seg;
+              if (sg != seg) {
+                seg = sg;
+                tt = lora_ranks(lacc, hr, sg, lane);
+              }
 #pragma unroll
               for (int e = 0; e < 2; ++e) o[e] += lora_term(p, tt, nc + e);
             }
@@ -346,7 +371,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
       if (et == 0 && it == 0) stamp(5);
-      if (p.counters != nullptr) {
+      if (!LORA && p.counters != nullptr) {
         // split-K, in-kernel finalize: publish this item's partial tile (bar.sync ordered every consumer thread's stores
         // before this thread; its gpu-scope fence is cumulative over them - the pattern of a cooperative grid sync)
         epi_bar();
@@ -356,7 +381,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-    if (p.counters != nullptr) {
+    if (!LORA && p.counters != nullptr) {
       // ---- phase 2 (split-K only): the `splits` CTAs that hold the partials of one output tile each reduce 1/splits of
       // its rows, in the fixed order split 0..S-1 (bitwise reproducible), and apply bias / per-batch bias / residual.
       // Deadlock-free: the grid has at most one CTA per SM (all resident), and no CTA waits before ALL its own partials are
@@ -619,7 +644,6 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   p.splits = splits;
   p.kb_per_split = (int)ceil_div(p.kb_total, splits);
   MOS_CHECK_ARG((long long)p.kb_per_split * (splits - 1) < p.kb_total, "mos_gemm_bf16: empty split");
-  p.lora = lora ? 1 : 0;
   p.geglu = a->geglu;
   p.out_mode = a->out_mode;
   p.partial = a->partial;
@@ -685,17 +709,16 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   static bool configured = false;
   if (!configured) {
     configured = true;
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(gemm_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_DYN_SMEM));
   }
   // persistent: at most one CTA per SM; each CTA loops over its share of the (tile, split) work items
   const int units = p.total_items < num_sms ? p.total_items : num_sms;
-  if (f16)
-    MOS_CHECK_CUDA(launch_pdl(gemm_kernel<true>, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA,
-                              tmB, tmL, p));
-  else
-    MOS_CHECK_CUDA(launch_pdl(gemm_kernel<false>, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA,
-                              tmB, tmL, p));
+  auto kern = f16 ? (lora ? gemm_kernel<true, true> : gemm_kernel<true, false>)
+                  : (lora ? gemm_kernel<false, true> : gemm_kernel<false, false>);
+  MOS_CHECK_CUDA(launch_pdl(kern, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA, tmB, tmL, p));
   return MOS_OK;
 }
 
