@@ -344,7 +344,8 @@ int mos_lora_grad(const void* x, int64_t ldx, const void* dy, int64_t lddy, int6
 /* Attention regulariser (cal_attn_reg, trainer_edlora.py:263-313) restricted to the two concept-token columns.
  * One resolution group per call: pcols_host_ptrs = host array of L device pointers [B*heads, res*res, 2] (the
  * mos_attention_fwd_train outputs of the group's layers); mask fp32 [B, 1, MH, MW]; cm [B, res*res, 2] and
- * stats[8] = {max0, max1, argmax0, argmax1, n_zero, weighted loss, S0, S1} are outputs.  mos_attn_reg_grad turns them
+ * stats[8] = {max0, max1, ties0, ties1, n_zero, weighted loss, S0, S1} are outputs (ties_c = the number of elements equal
+ * to max_c, which share the max's gradient evenly, as torch's max() backward).  mos_attn_reg_grad turns them
  * into gcols [B, res*res, 2] (the gradient on every layer/head's probabilities of the group; zero if any group of
  * stats_all [ngroups][8] is NaN, the reference's skip rule :257); mos_attn_reg_total: out[0] = mse + valid attention
  * loss, out[1] = attention loss (NaN when skipped). */

@@ -449,7 +449,8 @@ __global__ void lora_grad_reduce_kernel(const float* __restrict__ partial, int n
 //   cm[b, n, c] = mean over (layers of the group x heads) of pcols_l[(b, h), n, c]
 //   y_c = cm_c / max(cm_c)  (max over the whole batch);  gt = nearest-resized mask
 //   loss = w * ( full ? mean((y_1 - gt)^2) : mean_{gt==0} y_1   +   mean_{gt==0} y_0 )
-// stats[8] per group = {max0, max1, argmax0, argmax1 (int bits), nzero, loss, S0, S1}, S_c = sum_i g_i x_i (g = dloss/dy)
+// stats[8] per group = {max0, max1, T0, T1, nzero, loss, S0, S1}, S_c = sum_i g_i x_i (g = dloss/dy), T_c = the number of
+// elements equal to max_c (torch's max() backward splits the gradient of the maximum evenly among them)
 struct RegPtrs {
   const float* p[8];
 };
@@ -478,52 +479,42 @@ __device__ __forceinline__ float reg_gt(const float* __restrict__ mask, int b, i
 __global__ void __launch_bounds__(1024)
 attnreg_reduce_kernel(const float* __restrict__ cm, const float* __restrict__ mask, int B, int res, int MH, int MW,
                       int full_identity, float weight, float* __restrict__ stats) {
-  __shared__ float sv[4][32];
-  __shared__ int si[2][32];
+  __shared__ float sv[5][32];
   __shared__ float bc[8];
   pdl_wait();
   pdl_launch_dependents();
   const int N = res * res, total = B * N;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  // ---- phase 1: max / argmax per column, number of zero mask pixels
+  // ---- phase 1: max per column, number of zero mask pixels
   float m0 = -INFINITY, m1 = -INFINITY, nz = 0.f;
-  int a0 = 0x7fffffff, a1 = 0x7fffffff;
   for (int i = threadIdx.x; i < total; i += blockDim.x) {
-    const float x0 = cm[2 * i], x1 = cm[2 * i + 1];
-    if (x0 > m0) { m0 = x0; a0 = i; }
-    if (x1 > m1) { m1 = x1; a1 = i; }
+    m0 = fmaxf(m0, cm[2 * i]);
+    m1 = fmaxf(m1, cm[2 * i + 1]);
     nz += (reg_gt(mask, i / N, i % N, res, MH, MW) == 0.f) ? 1.f : 0.f;
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {
-    const float o0 = __shfl_xor_sync(0xffffffffu, m0, d), o1 = __shfl_xor_sync(0xffffffffu, m1, d);
-    const int b0 = __shfl_xor_sync(0xffffffffu, a0, d), b1 = __shfl_xor_sync(0xffffffffu, a1, d);
-    if (o0 > m0 || (o0 == m0 && b0 < a0)) { m0 = o0; a0 = b0; }
-    if (o1 > m1 || (o1 == m1 && b1 < a1)) { m1 = o1; a1 = b1; }
+    m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, d));
+    m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, d));
     nz += __shfl_xor_sync(0xffffffffu, nz, d);
   }
-  if (lane == 0) {
-    sv[0][warp] = m0; sv[1][warp] = m1; sv[2][warp] = nz;
-    si[0][warp] = a0; si[1][warp] = a1;
-  }
+  if (lane == 0) { sv[0][warp] = m0; sv[1][warp] = m1; sv[2][warp] = nz; }
   __syncthreads();
   if (threadIdx.x == 0) {
     float M0 = -INFINITY, M1 = -INFINITY, Z = 0.f;
-    int A0 = 0x7fffffff, A1 = 0x7fffffff;
     for (int w = 0; w < nw; ++w) {
-      if (sv[0][w] > M0 || (sv[0][w] == M0 && si[0][w] < A0)) { M0 = sv[0][w]; A0 = si[0][w]; }
-      if (sv[1][w] > M1 || (sv[1][w] == M1 && si[1][w] < A1)) { M1 = sv[1][w]; A1 = si[1][w]; }
+      M0 = fmaxf(M0, sv[0][w]);
+      M1 = fmaxf(M1, sv[1][w]);
       Z += sv[2][w];
     }
     bc[0] = M0; bc[1] = M1; bc[2] = Z;
     stats[0] = M0; stats[1] = M1;
-    stats[2] = __int_as_float(A0); stats[3] = __int_as_float(A1);
     stats[4] = Z;
   }
   __syncthreads();
   const float M0 = bc[0], M1 = bc[1], Z = bc[2];
-  // ---- phase 2: loss and S_c = sum_i g_i x_i
-  float ls = 0.f, s0 = 0.f, s1 = 0.f;
+  // ---- phase 2: loss, S_c = sum_i g_i x_i and the tie counts T_c
+  float ls = 0.f, s0 = 0.f, s1 = 0.f, t0 = 0.f, t1 = 0.f;
   for (int i = threadIdx.x; i < total; i += blockDim.x) {
     const float x0 = cm[2 * i], x1 = cm[2 * i + 1];
     const float gt = reg_gt(mask, i / N, i % N, res, MH, MW);
@@ -540,26 +531,32 @@ attnreg_reduce_kernel(const float* __restrict__ cm, const float* __restrict__ ma
     ls += zero * y0 / Z;
     s0 += (zero / Z) * x0;
     s1 += g1 * x1;
+    t0 += (x0 == M0) ? 1.f : 0.f;
+    t1 += (x1 == M1) ? 1.f : 0.f;
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {
     ls += __shfl_xor_sync(0xffffffffu, ls, d);
     s0 += __shfl_xor_sync(0xffffffffu, s0, d);
     s1 += __shfl_xor_sync(0xffffffffu, s1, d);
+    t0 += __shfl_xor_sync(0xffffffffu, t0, d);
+    t1 += __shfl_xor_sync(0xffffffffu, t1, d);
   }
   __syncthreads();
-  if (lane == 0) { sv[0][warp] = ls; sv[1][warp] = s0; sv[2][warp] = s1; }
+  if (lane == 0) { sv[0][warp] = ls; sv[1][warp] = s0; sv[2][warp] = s1; sv[3][warp] = t0; sv[4][warp] = t1; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float a = 0.f, b = 0.f, c = 0.f;
-    for (int w = 0; w < nw; ++w) { a += sv[0][w]; b += sv[1][w]; c += sv[2][w]; }
+    float a = 0.f, b = 0.f, c = 0.f, u0 = 0.f, u1 = 0.f;
+    for (int w = 0; w < nw; ++w) { a += sv[0][w]; b += sv[1][w]; c += sv[2][w]; u0 += sv[3][w]; u1 += sv[4][w]; }
+    stats[2] = u0;
+    stats[3] = u1;
     stats[5] = weight * a;   // NaN when Z == 0, as the reference's mean over an empty selection
     stats[6] = b;
     stats[7] = c;
   }
 }
 
-// gcols[b, n, c] = valid * w * (g_c / max_c - [i == argmax_c] S_c / max_c^2) / (heads * L)
+// gcols[b, n, c] = valid * w * (g_c / max_c - [x_c == max_c] S_c / (max_c^2 T_c)) / (heads * L)
 __global__ void attnreg_grad_kernel(const float* __restrict__ cm, const float* __restrict__ mask, int B, int res,
                                     int MH, int MW, int full_identity, float weight, const float* __restrict__ stats_all,
                                     int ngroups, int group, int L, int heads, float grad_scale,
@@ -572,16 +569,15 @@ __global__ void attnreg_grad_kernel(const float* __restrict__ cm, const float* _
   bool valid = true;
   for (int g = 0; g < ngroups; ++g) valid = valid && (stats_all[g * 8 + 4] > 0.f);
   const float* st = stats_all + group * 8;
-  const float M0 = st[0], M1 = st[1], Z = st[4], S0 = st[6], S1 = st[7];
-  const int A0 = __float_as_int(st[2]), A1 = __float_as_int(st[3]);
+  const float M0 = st[0], M1 = st[1], T0 = st[2], T1 = st[3], Z = st[4], S0 = st[6], S1 = st[7];
   const float gt = reg_gt(mask, i / N, i % N, res, MH, MW);
   const float zero = (gt == 0.f) ? 1.f : 0.f;
-  const float x1 = cm[2 * i + 1];
+  const float x0 = cm[2 * i], x1 = cm[2 * i + 1];
   const float g1 = full_identity ? 2.0f * (x1 / M1 - gt) / (float)total : zero / Z;
   const float g0 = zero / Z;
   const float k = valid ? grad_scale * weight / (float)(heads * L) : 0.f;
-  float d0 = g0 / M0 - (i == A0 ? S0 / (M0 * M0) : 0.f);
-  float d1 = g1 / M1 - (i == A1 ? S1 / (M1 * M1) : 0.f);
+  float d0 = g0 / M0 - (x0 == M0 ? S0 / (M0 * M0 * T0) : 0.f);
+  float d1 = g1 / M1 - (x1 == M1 ? S1 / (M1 * M1 * T1) : 0.f);
   if (!valid) d0 = d1 = 0.f;   // avoid 0 * NaN
   gcols[2 * i] = k * d0;
   gcols[2 * i + 1] = k * d1;

@@ -14,6 +14,12 @@ def rel_l2(a, b):
     return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
 
 
+def rel_l2_64(a, b):
+    """rel_l2 evaluated in float64, for fp32 kernels against float64 references"""
+    a, b = a.double(), b.double()
+    return ((a - b).norm() / b.norm().clamp_min(1e-300)).item()
+
+
 def mk(shape, dev, scale=1.0, seed=0, dtype=torch.bfloat16):
     g = torch.Generator(device='cpu').manual_seed(seed)
     return (torch.randn(shape, generator=g) * scale).to(dev).to(dtype)
