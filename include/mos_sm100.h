@@ -336,7 +336,8 @@ int mos_add_noise(const float* x0, const float* noise, const int32_t* timesteps,
 /* LoRA gradients of y = x W^T + alpha (x D^T) U^T (edlora.py:244-246):  d_up [N, 4] (+)= alpha dY^T (x D^T),
  * d_down [4, K] (+)= alpha (dY U)^T x.  x bf16 [M, K], dy bf16 [M, N], down fp32 [4, K], up fp32 [N, 4];
  * workspace >= 128 * 4 * (K + N) floats (at most 128 row slabs, one partial each); fixed-order reduction (bitwise
- * reproducible). */
+ * reproducible).  Any K, N (multiples of 8): D and U are staged in shared memory when they fit, and read from global
+ * memory by the same arithmetic otherwise (e.g. K = 1280, N = 10240). */
 int mos_lora_grad(const void* x, int64_t ldx, const void* dy, int64_t lddy, int64_t M, int32_t K, int32_t N,
                   const float* down, const float* up, float alpha, float* workspace, int64_t workspace_floats,
                   int32_t accumulate, float* d_down, float* d_up, void* stream);

@@ -293,28 +293,39 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, int DP, 
 //           FMAs per row; the 4 row groups are summed in a fixed order through smem
 // and writes its partial [4K + 4N]; lora_grad_reduce_kernel sums the <= 128 partials in a fixed order (bitwise
 // reproducible).
+// STAGE = false is the wide-layer variant (e.g. the GEGLU projection 1280 -> 10240, where D and U alone need 210 KB): D and
+// U are read from global memory (L1 / L2 resident, 4 (K + N) floats) instead of being staged, and nothing else changes,
+// so both variants give the same bits for any shape both accept.
 constexpr int LG_THREADS = 256;
 constexpr int LG_MAX_BLOCKS = 128;
+constexpr long long LG_SMEM_MAX = 200 * 1024;
 
+template <bool STAGE>
 __global__ void __launch_bounds__(LG_THREADS)
 lora_grad_partial_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __nv_bfloat16* __restrict__ dy,
                          long long lddy, long long M, int K, int N, const float* __restrict__ down,
                          const float* __restrict__ up, int R, float* __restrict__ partial) {
   extern __shared__ float lg_smem[];
-  float* sD = lg_smem;                 // [4][K]
-  float* sU = sD + 4 * K;              // [N][4]
-  float* ts = sU + 4 * N;              // [R][8]: t[0..3], s[0..3]
-  float* red = ts + (long long)R * 8;  // [4 groups][32 values][64 lanes]
+  float* ts = STAGE ? lg_smem + 4 * K + 4 * N : lg_smem;   // [R][8]: t[0..3], s[0..3]
+  float* red = ts + (long long)R * 8;                      // [4 groups][32 values][64 lanes]
+  const float* sD = down;              // [4][K]
+  const float* sU = up;                // [N][4]
   pdl_wait();
   pdl_launch_dependents();
   const int tid = threadIdx.x;
   const long long m0 = (long long)blockIdx.x * R;
   const int rows = (int)min((long long)R, M - m0);
-  for (int i = tid * 4; i < 4 * K; i += LG_THREADS * 4)
-    *reinterpret_cast<float4*>(sD + i) = __ldg(reinterpret_cast<const float4*>(down + i));
-  for (int i = tid * 4; i < 4 * N; i += LG_THREADS * 4)
-    *reinterpret_cast<float4*>(sU + i) = __ldg(reinterpret_cast<const float4*>(up + i));
-  __syncthreads();
+  if (STAGE) {
+    float* stD = lg_smem;
+    float* stU = stD + 4 * K;
+    for (int i = tid * 4; i < 4 * K; i += LG_THREADS * 4)
+      *reinterpret_cast<float4*>(stD + i) = __ldg(reinterpret_cast<const float4*>(down + i));
+    for (int i = tid * 4; i < 4 * N; i += LG_THREADS * 4)
+      *reinterpret_cast<float4*>(stU + i) = __ldg(reinterpret_cast<const float4*>(up + i));
+    sD = stD;
+    sU = stU;
+    __syncthreads();
+  }
   // ---- step 1: t = x D^T, s = dY U for every row of the slab.  Thread = (row, part): with R <= 128 rows the 256 threads
   // split every row's columns P = 256 / R ways (chunk c goes to part c mod P); partial dots are summed in a fixed order.
   const int P = R >= LG_THREADS ? 1 : LG_THREADS / R;
@@ -700,14 +711,21 @@ extern "C" int mos_lora_grad(const void* x, int64_t ldx, const void* dy, int64_t
   const int nb = (int)ceil_div(M, R);
   MOS_CHECK_ARG((long long)nb * 4 * (K + N) <= workspace_floats, "mos_lora_grad: workspace too small (need %lld floats)",
                 (long long)nb * 4 * (K + N));
-  const size_t smem = (size_t)(4LL * K + 4LL * N + R * 8 + 4 * 32 * 64) * sizeof(float);
-  MOS_CHECK_ARG(smem <= 200 * 1024, "mos_lora_grad: K + N = %d too large for the shared-memory staging", K + N);
+  // D and U are staged in shared memory whenever they fit next to the slab's t / s rows and the reduction buffer; wider
+  // layers read them from global memory (same arithmetic, same bits)
+  const size_t smem_work = (size_t)(R * 8 + 4 * 32 * 64) * sizeof(float);
+  const size_t smem_staged = smem_work + (size_t)(4LL * K + 4LL * N) * sizeof(float);
+  const bool stage = smem_staged <= (size_t)LG_SMEM_MAX;
   static bool configured = false;
   if (!configured) {
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(lora_grad_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(lora_grad_partial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)LG_SMEM_MAX));
+    MOS_CHECK_CUDA(cudaFuncSetAttribute(lora_grad_partial_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)LG_SMEM_MAX));
     configured = true;
   }
-  MOS_CHECK_CUDA(launch_pdl(lora_grad_partial_kernel, dim3(nb), dim3(LG_THREADS), smem, STREAM(stream),
+  MOS_CHECK_CUDA(launch_pdl(stage ? lora_grad_partial_kernel<true> : lora_grad_partial_kernel<false>, dim3(nb),
+                            dim3(LG_THREADS), stage ? smem_staged : smem_work, STREAM(stream),
                             reinterpret_cast<const __nv_bfloat16*>(x), (long long)ldx,
                             reinterpret_cast<const __nv_bfloat16*>(dy), (long long)lddy, (long long)M, (int)K, (int)N, down,
                             up, (int)R, workspace));

@@ -4,21 +4,31 @@
 (`init_new_concept`, `set_finetune_cfg`, `get_params_to_optimize`, `get_all_concept_token_ids`, `forward`,
 `delta_state_dict`, `load_delta_state_dict`) and its checkpoint layout ({'new_concept_embedding', 'text_encoder', 'unet'},
 keys f'{module}.lora_down.weight' / '.lora_up.weight', :371-378), and trains all THREE parameter groups of :82-139 — the
-new-concept embedding rows, the CLIPAttention LoRA and the UNet Attention LoRA — in one captured CUDA graph: text encoder
+new-concept embedding rows, the text-encoder LoRA and the UNet LoRA — in one captured CUDA graph: text encoder
 forward -> UNet forward -> masked MSE + attention regulariser -> UNet backward -> text encoder backward
 (mos_b200/train_engine.py + mos_b200/clip_train_engine.py).  The gradients land in ONE flat fp32 buffer (the payload of the
 step's single NCCL all-reduce); there is no autograd graph to call `.backward()` on.  `forward` takes images (encoded by
 the GPU VAE engine, :203-204) or already encoded latents.
 
 `UNetLoRATrainer` is the latents-and-embeddings level trainer of the UNet LoRA group alone (text encoder frozen and run
-upstream)."""
+upstream).
+
+LoRA placement (`lora_cfg.where`, trainer_edlora.py:100-133): the UNet takes `Attention` or `Transformer2DModel`, the text
+encoder `CLIPAttention` or `CLIPEncoderLayer`, in any combination."""
 import math
 import re
 
 import torch
 
+from mos_b200.clip_train_engine import CLIP_WHERE
 from mos_b200.engine import ehs_to_layer_major
-from mos_b200.train_engine import TrainEngine
+from mos_b200.train_engine import UNET_WHERE, TrainEngine
+
+
+def _check_where(where, allowed, part):
+    if where not in allowed:
+        raise NotImplementedError(f"{part} lora_cfg.where: {where!r} is not one of the reference's placements {allowed}")
+    return where
 
 
 class UNetLoRATrainer:
@@ -51,26 +61,24 @@ class UNetLoRATrainer:
         if not (ucfg.get('enable_tuning') and ucfg.get('lora_cfg')):
             raise ValueError("finetune_cfg['unet'] must enable tuning with a lora_cfg")
         lora_cfg = dict(ucfg['lora_cfg'])
-        where = lora_cfg.pop('where')
-        if where != 'Attention':
-            raise NotImplementedError("lora_cfg.where: only 'Attention' (the shipped ED-LoRA configs) is supported")
+        self.where = _check_where(lora_cfg.pop('where'), UNET_WHERE, 'unet')
         self.rank = int(lora_cfg.get('rank', 4))
         self.alpha = float(lora_cfg.get('alpha', 1.0))
         if not 1 <= self.rank <= 4:
             raise ValueError('LoRA rank must be in 1..4 (fused epilogue)')
         self.unet_lr = float(ucfg['lr'])
         H, W = self.latent_size
-        probe_names = TrainEngine.lora_module_names.__get__(_NameProbe(self._topo))()
+        probe_names = TrainEngine.lora_module_names.__get__(_NameProbe(self._topo, self.where))()
         if lora_state is None:
             lora_state = self._init_lora(probe_names)
         self.engine = TrainEngine(self._sd, self.batch, H, W, lora=lora_state, lora_alpha=self.alpha,
                                   attn_reg_weight=self.attn_reg_weight, reg_full_identity=self.reg_full_identity,
-                                  lr=self.unet_lr, device=self.device, **self._topo)
+                                  lr=self.unet_lr, device=self.device, where=self.where, **self._topo)
         self._sd = None
         self.params_to_optimize_iterator = [{'params': [self.engine.state.params], 'lr': self.unet_lr}]
 
     def _init_lora(self, names):
-        """LoRALinearLayer init (edlora.py:238-239): down ~ kaiming_uniform(a=sqrt(5)), up = 0."""
+        """LoRALinearLayer init (edlora.py:238-239): down ~ kaiming_uniform(a=sqrt(5)) (bound 1/sqrt(fan_in)), up = 0."""
         state = {}
         for m in names:
             w = self._sd[m + '.weight']
@@ -149,22 +157,16 @@ class UNetLoRATrainer:
         views = self.engine.lora_views
         if len(unet) != 2 * len(views):
             raise ValueError(f'checkpoint has {len(unet)} unet tensors, the model has {2 * len(views)} LoRA tensors')
-        for m, (D, U, _, _, K, N) in views.items():
-            d = unet[f'{m}.lora_down.weight'].to(self.device, torch.float32).reshape(-1, K)
-            u = unet[f'{m}.lora_up.weight'].to(self.device, torch.float32).reshape(N, -1)
-            D.zero_()
-            U.zero_()
-            D[:d.shape[0]] = d
-            U[:, :u.shape[1]] = u
-        self.engine.refresh_lora()
+        self.engine.load_lora_state_dict(unet)
 
 
 class _NameProbe:
     """enough of the engine surface for TrainEngine.lora_module_names before the engine exists"""
 
-    def __init__(self, topo):
+    def __init__(self, topo, where='Attention'):
         from mos_b200.engine import cross_attention_names
         self.xattn_names = cross_attention_names(topo.get('block_out', (320, 640, 1280, 1280)), topo.get('layers', 2))
+        self.where = where
 
 
 # ================================================================================================ full ED-LoRA trainer
@@ -256,8 +258,8 @@ class EDLoRATrainer:
                                       '(text_embedding, text_encoder LoRA, unet LoRA); use UNetLoRATrainer for the UNet '
                                       'group alone')
         tcfg, ucfg = dict(tx['lora_cfg']), dict(un['lora_cfg'])
-        if tcfg.pop('where') != 'CLIPAttention' or ucfg.pop('where') != 'Attention':
-            raise NotImplementedError("lora_cfg.where: 'CLIPAttention' / 'Attention' (every shipped ED-LoRA config) only")
+        self.text_where = _check_where(tcfg.pop('where'), CLIP_WHERE, 'text_encoder')
+        self.unet_where = _check_where(ucfg.pop('where'), UNET_WHERE, 'unet')
         for c in (tcfg, ucfg):
             if not 1 <= int(c.get('rank', 4)) <= 4:
                 raise ValueError('LoRA rank must be in 1..4 (fused epilogue)')
@@ -283,11 +285,10 @@ class EDLoRATrainer:
                     cross_dim=c.cross_attention_dim)
         usd = {k: v.detach() for k, v in self.unet.state_dict().items()}
         tsd = self.text_encoder.state_dict()
-        probe = _NameProbe(topo)
+        probe = _NameProbe(topo, self.unet_where)
         unet_names = TrainEngine.lora_module_names.__get__(probe)()
         n_layers = 1 + max(int(k.split('.layers.')[1].split('.')[0]) for k in tsd if '.layers.' in k)
-        text_names = [f'text_model.encoder.layers.{i}.self_attn.{p}' for i in range(n_layers)
-                      for p in ('q_proj', 'k_proj', 'v_proj', 'out_proj')]
+        text_names = CLIPTrainEngine.module_names(n_layers, self.text_where)
         ulora, tlora = {}, {}
         for m in unet_names:                                   # LoRALinearLayer init: down kaiming, up zeros (:238-239)
             w = usd[m + '.weight']
@@ -300,7 +301,8 @@ class EDLoRATrainer:
         ids = self.get_all_concept_token_ids()
         C = tsd['text_model.embeddings.token_embedding.weight'].shape[1]
         heads = getattr(self.text_encoder, 'hf_config', {}).get('num_attention_heads', 12)
-        n_text = CLIPTrainEngine.lora_param_count(n_layers, C, heads * 80)
+        n_inner = tsd['text_model.encoder.layers.0.mlp.fc1.weight'].shape[0]
+        n_text = CLIPTrainEngine.lora_param_count(n_layers, C, heads * 80, where=self.text_where, inner=n_inner)
         n_unet = sum(4 * (usd[m + '.weight'].reshape(usd[m + '.weight'].shape[0], -1).shape[1] + usd[m + '.weight'].shape[0])
                      for m in unet_names)
         self.state = FlatTrainState(len(ids), C, n_text, n_unet, lrs=self.lrs, device=self.device)
@@ -308,11 +310,12 @@ class EDLoRATrainer:
         self.engine = TrainEngine(usd, batch, H, W, lora=ulora, lora_alpha=self.unet_alpha,
                                   attn_reg_weight=self.attn_reg_weight, reg_full_identity=self.reg_full_identity,
                                   state=self.state, state_offset=self.state.group_end[1], text_grad=True,
-                                  device=self.device, **topo)
+                                  device=self.device, where=self.unet_where, **topo)
         n_x = len(self.engine.xattn_names)
         self.text_engine = CLIPTrainEngine(tsd, n_x * batch, lora=tlora, lora_alpha=self.text_alpha,
                                            concept_token_ids=ids, state=self.state, emb_offset=0,
-                                           lora_offset=self.state.group_end[0], device=self.device, heads=heads)
+                                           lora_offset=self.state.group_end[0], device=self.device, heads=heads,
+                                           where=self.text_where)
         self.engine.attach_text_engine(self.text_engine)
         self._batch = batch
         if self._loaded is not None:
@@ -420,11 +423,5 @@ class EDLoRATrainer:
             self.text_engine.load_lora_state_dict(delta['text_encoder'])
         unet = delta.get('unet') or {}
         if unet:
-            for m, (D, U, _, _, K, N) in self.engine.lora_views.items():
-                d = unet[f'{m}.lora_down.weight'].to(self.device, torch.float32).reshape(-1, K)
-                u = unet[f'{m}.lora_up.weight'].to(self.device, torch.float32).reshape(N, -1)
-                D.zero_()
-                U.zero_()
-                D[:d.shape[0]] = d
-                U[:, :u.shape[1]] = u
+            self.engine.load_lora_state_dict(unet)
         self.refresh()

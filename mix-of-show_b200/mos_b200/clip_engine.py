@@ -3,14 +3,16 @@
 Owns the `text_encoder(input_ids)[0]` call the reference makes at mixofshow/pipelines/pipeline_edlora.py:133-145,
 trainer_edlora.py:220-234 and gradient_fusion.py:182-199 (transformers `CLIPTextModel`: token + position embeddings,
 12 pre-LN layers of causal self-attention and a quick-GELU MLP, final LayerNorm), with the ED-LoRA of `where: CLIPAttention`
-(q_proj / k_proj / v_proj / out_proj, trainer_edlora.py:107-118) fused into the projection GEMMs exactly as in the UNet.
+(q_proj / k_proj / v_proj / out_proj, trainer_edlora.py:107-118) fused into the projection GEMMs exactly as in the UNet;
+with `where: CLIPEncoderLayer` the LoRA of mlp.fc1 / mlp.fc2 is fused into the MLP GEMMs the same way.
 
 Shapes are bent to the GEMM kernel's 160-column tiles without touching the arithmetic:
   * hidden states live in [M, 800] buffers (768 real columns, the rest stays zero: zero weight rows / bias);
   * the 12 heads of 64 dims run as head_dim 80 (16 zero columns per head in q, k, v; `scale` stays 64^-0.5), so the fused
     q|k|v projection has N = 3 * 12 * 80 = 2880 = 18 tiles and feeds the existing head-split epilogue and the d = 80
     attention kernel (causal variant); out_proj reads K = 960 with zero weight columns at the pads;
-  * fc1 is padded 3072 -> 3200 (quick-GELU(0) = 0), fc2 reads K = 3200.
+  * fc1 is padded 3072 -> 3200 (quick-GELU(0) = 0), fc2 reads K = 3200; their LoRA up rows / down columns are padded
+    the same way with zeros.
 There is no CPU / PyTorch fallback: every arithmetic op is a C-ABI call.
 """
 import torch
@@ -31,6 +33,7 @@ class CLIPTextEngine:
                  prefix='text_model.', eps=1e-5):
         """state_dict: transformers CLIPTextModel parameter names (fp32).  lora: {f'{module}.lora_down.weight' [r, 768],
         f'{module}.lora_up.weight' [768, r]} with module = 'text_model.encoder.layers.{i}.self_attn.{q,k,v,out}_proj'
+        and optionally 'text_model.encoder.layers.{i}.mlp.fc{1,2}' ([r, 768] / [3072, r] and [r, 3072] / [768, r])
         (EDLoRATrainer.delta_state_dict()['text_encoder'], trainer_edlora.py:371-378); rank <= 4.
         n_seq: number of 77-token sequences per call (16 per prompt for the layer-wise embeddings)."""
         self.dev = torch.device(device)
@@ -139,16 +142,43 @@ class CLIPTextEngine:
             ent['out'].update(lora_down=d16.to(BF16).contiguous(), lora_up=u4.contiguous(), lora_seg=Cp)
         # ---- MLP: fc1 N padded to Ip, fc2 K = Ip, N padded to Cp
         W1 = torch.zeros(self.Ip, C, device=self.dev)
-        W1[:self.I] = f32(L + 'mlp.fc1.weight')
+        W1[:self.I] = self._mlp_weight(L + 'mlp.fc1', f32)
         b1 = torch.zeros(self.Ip, device=self.dev)
         b1[:self.I] = f32(L + 'mlp.fc1.bias')
         ent['fc1'] = {'W': W1.to(BF16).contiguous(), 'bias': b1.contiguous()}
         W2 = torch.zeros(Cp, self.Ip, device=self.dev)
-        W2[:C, :self.I] = f32(L + 'mlp.fc2.weight')
+        W2[:C, :self.I] = self._mlp_weight(L + 'mlp.fc2', f32)
         b2 = torch.zeros(Cp, device=self.dev)
         b2[:C] = f32(L + 'mlp.fc2.bias')
         ent['fc2'] = {'W': W2.to(BF16).contiguous(), 'bias': b2.contiguous()}
+        pair = self._lora_pair(L + 'mlp.fc1') if self._merge is None else None
+        if pair is not None:                 # down [r, 768] as is, up rows padded 3072 -> 3200
+            r = pair[0].shape[0]
+            assert r <= 4, 'LoRA rank > 4 is not supported by the fused epilogue'
+            d16 = torch.zeros(16, C, device=self.dev)
+            d16[:r] = pair[0]
+            u4 = torch.zeros(self.Ip, 4, device=self.dev)
+            u4[:self.I, :r] = pair[1] * self.alpha
+            ent['fc1'].update(lora_down=d16.to(BF16).contiguous(), lora_up=u4.contiguous(), lora_seg=self.Ip)
+        pair = self._lora_pair(L + 'mlp.fc2') if self._merge is None else None
+        if pair is not None:                 # down columns padded 3072 -> 3200, up rows 768 -> 800
+            r = pair[0].shape[0]
+            assert r <= 4, 'LoRA rank > 4 is not supported by the fused epilogue'
+            d16 = torch.zeros(16, self.Ip, device=self.dev)
+            d16[:r, :self.I] = pair[0]
+            u4 = torch.zeros(Cp, 4, device=self.dev)
+            u4[:C, :r] = pair[1] * self.alpha
+            ent['fc2'].update(lora_down=d16.to(BF16).contiguous(), lora_up=u4.contiguous(), lora_seg=Cp)
         self.w[i] = ent
+
+    def _mlp_weight(self, m, f32):
+        """fc1 / fc2 weight, with a merged LoRA folded in (merge_lora_into_weight, gradient_fusion.py:99-143)"""
+        W = f32(m + '.weight')
+        if self._merge is not None:
+            pair = self._lora_pair(m)
+            if pair is not None:
+                W = W + self.alpha * (pair[1] @ pair[0])
+        return W
 
     # ------------------------------------------------------------------------------------------ forward
     def buf(self, name, shape, dtype=BF16, zero=False):

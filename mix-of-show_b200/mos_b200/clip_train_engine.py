@@ -13,10 +13,15 @@ Sequence order: the 16 layer-wise prompts of a sample are laid out LAYER-MAJOR (
 the engine's output [16 * B * 77, 768] IS the UNet engine's `in_ehs` [16, B, 77, 768] and d(in_ehs) IS this engine's output
 gradient: no gather / scatter between the two engines.
 
-Flat parameter layout of a projection LoRA (padded to the GEMM shapes of clip_engine.py; pads are zero and stay zero):
+With `where: CLIPEncoderLayer` (trainer_edlora.py:100-112) mlp.fc1 / mlp.fc2 of every layer are trained too.
+
+Flat parameter layout of a LoRA (padded to the GEMM shapes of clip_engine.py; pads are zero and stay zero: their gradients
+are exactly zero, so AdamW never moves them):
     q / k / v : down [4, 768], up [960, 4]   (12 heads of 64 dims run as 80: rows h*80+64 .. h*80+79 are pads)
     out_proj  : down [4, 960] (pad columns as above), up [768, 4]
-`lora_state_dict()` / `load_lora_state_dict()` convert to / from the reference's [r, 768] / [768, r] checkpoint tensors.
+    mlp.fc1   : down [4, 768], up [3200, 4]  (rows 3072 .. 3199 are pads)
+    mlp.fc2   : down [4, 3200] (columns 3072 .. 3199 are pads), up [768, 4]
+`lora_state_dict()` / `load_lora_state_dict()` convert to / from the reference's checkpoint tensors ([r, in] / [out, r]).
 """
 import torch
 
@@ -25,20 +30,25 @@ from ._lib import MOS_SEG_ROWS
 from .clip_engine import BF16, PROJ, CLIPTextEngine, _r
 
 F32 = torch.float32
+CLIP_WHERE = ('CLIPAttention', 'CLIPEncoderLayer')
 
 
 class CLIPTrainEngine(CLIPTextEngine):
     def __init__(self, state_dict, n_seq, *, lora, lora_alpha=1.0, concept_token_ids=(), state=None, emb_offset=0,
-                 lora_offset=None, **kw):
+                 lora_offset=None, where='CLIPAttention', **kw):
         """lora: {f'{module}.lora_down.weight' [r,768], f'{module}.lora_up.weight' [768,r]} for every q/k/v/out_proj of
         every layer (rank <= 4).  concept_token_ids: rows of the token-embedding table that are trained.
         state: dp.FlatTrainState to live in (parameters / gradients are views of it): the embedding rows at
-        `emb_offset`, the LoRA block at `lora_offset`; None = a private state."""
+        `emb_offset`, the LoRA block at `lora_offset`; None = a private state.
+        where: the LoRA placement (CLIP_WHERE); `lora` must hold a pair for every module of lora_module_names()."""
+        if where not in CLIP_WHERE:
+            raise ValueError(f'where: {where!r} is not one of {CLIP_WHERE}')
+        self.where = where
         super().__init__(state_dict, n_seq, lora=lora, lora_alpha=lora_alpha, **kw)
         assert self.lora is not None, 'training needs an un-merged LoRA'
         self.concept_ids = [int(i) for i in concept_token_ids]
         R, C = len(self.concept_ids), self.C
-        n_lora = self.lora_param_count(self.n_layers, C, self.Ca)
+        n_lora = self.lora_param_count(self.n_layers, C, self.Ca, where=where, inner=self.I)
         if state is None:
             from .dp import FlatTrainState
             state = FlatTrainState(R, C, n_lora, 0, device=self.dev)
@@ -56,12 +66,34 @@ class CLIPTrainEngine(CLIPTextEngine):
         self.saved = []
 
     @staticmethod
-    def lora_param_count(n_layers, C, Ca):
-        return n_layers * (3 * (4 * C + 4 * Ca) + (4 * Ca + 4 * C))
+    def lora_param_count(n_layers, C, Ca, where='CLIPAttention', inner=3072):
+        """floats of the flat LoRA block (rank-4 slots, pads included)"""
+        n = 3 * (4 * C + 4 * Ca) + (4 * Ca + 4 * C)
+        if where == 'CLIPEncoderLayer':
+            Ip = _r(inner, 160)
+            n += (4 * C + 4 * Ip) + (4 * Ip + 4 * C)
+        return n_layers * n
+
+    @staticmethod
+    def module_names(n_layers, where='CLIPAttention', prefix='text_model.'):
+        """the modules that carry a LoRA, layer by layer (flat-state order)"""
+        mlp = ('mlp.fc1', 'mlp.fc2') if where == 'CLIPEncoderLayer' else ()
+        return [f'{prefix}encoder.layers.{i}.{p}' for i in range(n_layers)
+                for p in tuple('self_attn.' + q for q in PROJ) + mlp]
 
     # ------------------------------------------------------------------------------------------ LoRA state
     def lora_module_names(self):
-        return [f'{self.pre}encoder.layers.{i}.self_attn.{p}' for i in range(self.n_layers) for p in PROJ]
+        return self.module_names(self.n_layers, self.where, self.pre)
+
+    def _lora_shape(self, m):
+        """(K, N) of module m's flat LoRA (down [4, K], up [N, 4])"""
+        if m.endswith('out_proj'):
+            return self.Ca, self.C
+        if m.endswith('fc1'):
+            return self.C, self.Ip
+        if m.endswith('fc2'):
+            return self.Ip, self.C
+        return self.C, self.Ca
 
     def _pad_heads_rows(self, U):        # [heads*d, r] -> [heads*dh, r]
         out = torch.zeros(self.heads, self.dh, U.shape[1], device=self.dev)
@@ -80,9 +112,9 @@ class CLIPTrainEngine(CLIPTextEngine):
         for m in self.lora_module_names():
             kd = f'{m}.lora_down.weight'
             if kd not in lora:
-                raise ValueError(f'training needs a LoRA pair on every CLIPAttention projection; missing {kd}')
+                raise ValueError(f'training needs a LoRA pair on every module of `where: {self.where}`; missing {kd}')
             is_out = m.endswith('out_proj')
-            K, N = (Ca, C) if is_out else (C, Ca)
+            K, N = self._lora_shape(m)
             D = self.state.params[off:off + 4 * K].view(4, K)
             gD = self.state.grads[off:off + 4 * K].view(4, K)
             off += 4 * K
@@ -92,6 +124,16 @@ class CLIPTrainEngine(CLIPTextEngine):
             self.lora_views[m] = (D, U, gD, gU, K, N)
             i = int(m.split('.layers.')[1].split('.')[0])
             ent = self.w[i]
+            mlp = m.rsplit('.', 1)[1] if '.mlp.' in m else None
+            if mlp is not None:
+                # backward GEMMs: fc1 dX [M, 800] (768 real columns), fc2 dX [M, 3200] = the widths of the packs below
+                bd = torch.zeros(16, N, device=self.dev, dtype=BF16)
+                bu = torch.zeros(Cp if mlp == 'fc1' else self.Ip, 4, device=self.dev)
+                keep += [bd, bu]
+                self.wb[f'{self.pre}encoder.layers.{i}.{mlp}'] = {'lora_down': bd, 'lora_up': bu, 'lora_seg': bu.shape[0]}
+                rows.append([D.data_ptr(), U.data_ptr(), K, N, ent[mlp]['lora_down'].data_ptr(),
+                             ent[mlp]['lora_up'].data_ptr(), bd.data_ptr(), bu.data_ptr()])
+                continue
             if is_out:
                 fdown = ent['out']['lora_down'].data_ptr()
                 fup = ent['out']['lora_up'].data_ptr()
@@ -114,11 +156,18 @@ class CLIPTrainEngine(CLIPTextEngine):
     def load_lora_state_dict(self, lora):
         """reference checkpoint tensors ([r, 768] / [768, r], trainer_edlora.py:371-378) -> padded flat layout."""
         for m, (D, U, _, _, K, N) in self.lora_views.items():
-            d = lora[f'{m}.lora_down.weight'].detach().to(self.dev, F32).reshape(-1, self.C)
-            u = lora[f'{m}.lora_up.weight'].detach().to(self.dev, F32).reshape(self.C, -1)
+            d = lora[f'{m}.lora_down.weight'].detach().to(self.dev, F32)
+            u = lora[f'{m}.lora_up.weight'].detach().to(self.dev, F32)
+            d, u = d.reshape(d.shape[0], -1), u.reshape(u.shape[0], -1)
             D.zero_()
             U.zero_()
-            if m.endswith('out_proj'):
+            if m.endswith('fc1'):
+                D[:d.shape[0]] = d
+                U[:self.I, :u.shape[1]] = u
+            elif m.endswith('fc2'):
+                D[:d.shape[0], :self.I] = d
+                U[:, :u.shape[1]] = u
+            elif m.endswith('out_proj'):
                 D[:d.shape[0]] = self._pad_heads_cols(d)
                 U[:, :u.shape[1]] = u
             else:
@@ -127,6 +176,10 @@ class CLIPTrainEngine(CLIPTextEngine):
         self.refresh_lora()
 
     def _unpad(self, m, D, U):
+        if m.endswith('fc1'):
+            return D, U[:self.I]
+        if m.endswith('fc2'):
+            return D[:, :self.I], U
         if m.endswith('out_proj'):
             return D.view(4, self.heads, self.dh)[:, :, :self.d].reshape(4, self.C), U
         return D, U.view(self.heads, self.dh, 4)[:, :self.d].reshape(self.C, 4)
@@ -169,9 +222,9 @@ class CLIPTrainEngine(CLIPTextEngine):
             W1 = ent['fc1']['W']                                     # [Ip, C]
             Wt = torch.zeros(Cp, self.Ip, device=self.dev, dtype=BF16)
             Wt[:C] = W1.t()
-            self.wb[L + 'fc1'] = {'W': Wt.contiguous(), 'bias': None}
+            self.wb.setdefault(L + 'fc1', {}).update(W=Wt.contiguous(), bias=None)
             W2 = ent['fc2']['W']                                     # [Cp, Ip]
-            self.wb[L + 'fc2'] = {'W': W2[:C].t().contiguous(), 'bias': None}        # [Ip, C]
+            self.wb.setdefault(L + 'fc2', {}).update(W=W2[:C].t().contiguous(), bias=None)        # [Ip, C]
 
     def _gemm_b(self, A, ent, out, *, M, residual=None, heads=None, lda=None):
         kw = {}
@@ -272,10 +325,17 @@ class CLIPTrainEngine(CLIPTextEngine):
             ent = self.w[i]
             L = f'{self.pre}encoder.layers.{i}.'
             # ---- MLP: x2 = x1 + fc2(quick_gelu(fc1(LN2(x1))))
+            mlp_lora = self.where == 'CLIPEncoderLayer'
+            if mlp_lora:        # fc2's input, quick_gelu(hpre), is recomputed instead of kept
+                h = self.buf('h', (M, self.Ip))
+                ops.quick_gelu_fwd(S['hpre'], h, M=M, C=self.Ip)
+                self._lora_grad(L + 'mlp.fc2', h, d_x, M, lddy=Cp)
             d_h = self.buf('g_h', (M, self.Ip))
             self._gemm_b(d_x, self.wb[L + 'fc2'], d_h, M=M, lda=Cp)                 # reduction over the 768 real columns
             d_hpre = self.buf('g_hpre', (M, self.Ip))
             ops.quick_gelu_bwd(S['hpre'], d_h, d_hpre, M=M, C=self.Ip)
+            if mlp_lora:
+                self._lora_grad(L + 'mlp.fc1', S['ln2'], d_hpre, M)
             d_ln = self.buf('g_ln', (M, Cp))
             self._gemm_b(d_hpre, self.wb[L + 'fc1'], d_ln, M=M)
             d_x1 = other

@@ -50,6 +50,16 @@ def cross_attention_names(block_out=(320, 640, 1280, 1280), layers=2):
     return names
 
 
+def geglu_perm(n):
+    """Row order of the packed GEGLU projection (n = 2H output rows): for every 160-column output tile, 80 rows of the value
+    half followed by the matching 80 rows of the gate half, so that the fused epilogue finds both halves of an output
+    column in one tile.  packed = natural[perm]."""
+    half = n // 2
+    assert half % 80 == 0
+    return torch.cat([torch.cat([torch.arange(80 * t, 80 * t + 80), half + torch.arange(80 * t, 80 * t + 80)])
+                      for t in range(half // 80)])
+
+
 class UNetEngine:
     def __init__(self, state_dict, batch, height, width, *, lora=None, lora_alpha=1.0, merge_lora=False,
                  device='cuda', block_out=(320, 640, 1280, 1280), layers=2, heads=8, cross_dim=768, n_text=77,
@@ -137,10 +147,7 @@ class UNetEngine:
         ent = {'N': N, 'K': K}
         perm = None
         if geglu:
-            half = N // 2
-            assert half % 80 == 0
-            perm = torch.cat([torch.cat([torch.arange(80 * t, 80 * t + 80), half + torch.arange(80 * t, 80 * t + 80)])
-                              for t in range(half // 80)]).to(self.dev)
+            perm = geglu_perm(N).to(self.dev)
             W = W[perm]
             bias = bias[perm] if bias is not None else None
         ent['W'] = W.to(self.ACT).contiguous()

@@ -4,8 +4,12 @@ group, train_edlora.py:57,129), built only from libmos_sm100 kernels.
 
 All base weights are frozen (trainer_edlora.py:88-90): the backward pass produces activation gradients (tensor-core
 GEMMs on transposed weight packs, flash-attention backward, GroupNorm / LayerNorm / GEGLU backward) and the rank-4 LoRA
-gradients of the 128 attention projections, accumulated into ONE flat fp32 buffer (dp.FlatTrainState) so that the
-data-parallel step needs a single all-reduce (SURVEY.md §8e).  The attention regulariser (cal_attn_reg, :263-313) only
+gradients, accumulated into ONE flat fp32 buffer (dp.FlatTrainState) so that the data-parallel step needs a single
+all-reduce (SURVEY.md §8e).  The LoRA placement is the reference's `where` (trainer_edlora.py:121-133): `Attention` = the
+128 attention projections; `Transformer2DModel` adds proj_in, proj_out (1x1 convs), ff.net.0.proj (GEGLU) and ff.net.2 of
+every transformer block.  The GEGLU projection's LoRA up lives in the flat state in the packed row order of its GEMM
+(engine.geglu_perm; AdamW is elementwise); `load_lora_state_dict` / `lora_state_dict` / `lora_grad_dict` speak the module's
+natural order.  The attention regulariser (cal_attn_reg, :263-313) only
 ever reads two key columns of the cross-attention maps, so the forward emits exactly those columns.
 
 VAE encoding and the CLIP text encoder (and with it the gradient w.r.t. the text embeddings) are §8f "next": this engine
@@ -18,10 +22,12 @@ import torch
 from . import ops
 from ._lib import MOS_SEG_ROWS
 from .dp import FlatTrainState
-from .engine import BF16, UNetEngine, _r
+from .engine import BF16, UNetEngine, _r, geglu_perm
 
 F32 = torch.float32
 _PROJ = ('to_q', 'to_k', 'to_v', 'to_out.0')
+UNET_WHERE = ('Attention', 'Transformer2DModel')
+_GEGLU = '.ff.net.0.proj'
 
 
 def _key(t):
@@ -30,11 +36,15 @@ def _key(t):
 
 class TrainEngine(UNetEngine):
     def __init__(self, state_dict, batch, height, width, *, lora, lora_alpha=1.0, attn_reg_weight=0.01,
-                 reg_full_identity=True, lr=1e-4, state=None, state_offset=0, text_grad=False, **kw):
-        """state / state_offset: a shared dp.FlatTrainState (and the offset of the UNet-LoRA block in it) when the text
+                 reg_full_identity=True, lr=1e-4, state=None, state_offset=0, text_grad=False, where='Attention', **kw):
+        """where: the LoRA placement (UNET_WHERE); `lora` must hold a pair for every module of lora_module_names().
+        state / state_offset: a shared dp.FlatTrainState (and the offset of the UNet-LoRA block in it) when the text
         encoder is trained in the same step (clip_train_engine.CLIPTrainEngine); None = a private state.
         text_grad: also produce d loss / d(text embeddings) into `self.d_ehs` (bf16 [16 * B * 77, 800], layer-major rows =
         the layout of `in_ehs`; the first 768 columns are the gradient) for the text encoder's backward."""
+        if where not in UNET_WHERE:
+            raise ValueError(f'where: {where!r} is not one of {UNET_WHERE}')
+        self.where = where
         self.use_train_graph = bool(kw.pop('use_graph', True))
         self._ext_state, self._state_off, self.text_grad = state, int(state_offset), bool(text_grad)
         self.tgraph = None
@@ -68,16 +78,33 @@ class TrainEngine(UNetEngine):
 
     # ------------------------------------------------------------------------------------------ LoRA state
     def lora_module_names(self):
+        """The modules that carry a LoRA, in the order of the reference's module walk (trainer_edlora.py:121-133)."""
+        whole = getattr(self, 'where', 'Attention') == 'Transformer2DModel'
         names = []
         for an in self.xattn_names:
             tb = an[:-len('.attn2')]
+            tn = tb[:-len('.transformer_blocks.0')]
+            if whole:
+                names.append(f'{tn}.proj_in')
             for a in ('attn1', 'attn2'):
                 for p in _PROJ:
                     names.append(f'{tb}.{a}.{p}')
+            if whole:
+                names += [tb + _GEGLU, f'{tb}.ff.net.2', f'{tn}.proj_out']
         return names
+
+    @property
+    def whole_block(self):
+        return self.where == 'Transformer2DModel'
 
     def _fwd_slot(self, m):
         """module name -> (forward pack key, segment index inside the fused pack)"""
+        if m.endswith('.proj_in') or m.endswith('.proj_out'):
+            return m, 0
+        if m.endswith(_GEGLU):
+            return m[:-len(_GEGLU)] + '.ff1', 0
+        if m.endswith('.ff.net.2'):
+            return m[:-len('.ff.net.2')] + '.ff2', 0
         if '.attn1.' in m:
             tb, p = m.split('.attn1.')
             if p == 'to_out.0':
@@ -90,13 +117,18 @@ class TrainEngine(UNetEngine):
             return f'{tb}.attn2.out', 0
         return f'{tb}.attn2.kv', ('to_k', 'to_v').index(p)
 
+    def _bwd_key(self, m):
+        """key of the transposed (dX) pack that carries module m's LoRA term: the attention projections have packs of their
+        own (the forward fuses q|k|v), the other modules share the forward pack's key"""
+        return m if ('.attn1.' in m or '.attn2.' in m) else self._fwd_slot(m)[0]
+
     def _build_lora_state(self, lora, lr):
         mods = self.lora_module_names()
         sizes = []
         for m in mods:
             kd = f'{m}.lora_down.weight'
             if kd not in lora:
-                raise ValueError(f'training needs a LoRA pair on every attention projection; missing {kd}')
+                raise ValueError(f'training needs a LoRA pair on every module of `where: {self.where}`; missing {kd}')
             K = lora[kd].reshape(lora[kd].shape[0], -1).shape[1]
             N = lora[f'{m}.lora_up.weight'].shape[0]
             sizes.append((K, N))
@@ -117,12 +149,6 @@ class TrainEngine(UNetEngine):
             U = self.state.params[off:off + 4 * N].view(N, 4)
             gU = self.state.grads[off:off + 4 * N].view(N, 4)
             off += 4 * N
-            d = lora[f'{m}.lora_down.weight'].detach().to(self.dev, F32).reshape(-1, K)
-            u = lora[f'{m}.lora_up.weight'].detach().to(self.dev, F32).reshape(N, -1)
-            D.zero_()
-            U.zero_()
-            D[:d.shape[0]] = d
-            U[:, :u.shape[1]] = u
             self.lora_views[m] = (D, U, gD, gU, K, N)
             key, seg = self._fwd_slot(m)
             ent = self.w[key]
@@ -139,26 +165,59 @@ class TrainEngine(UNetEngine):
                 bu = torch.zeros(kp, 4, device=self.dev)
                 keep += [bd, bu]
                 bdown, bup = bd.data_ptr(), bu.data_ptr()
-                self.wb[m] = {'N': kp, 'K': N, 'bias': None, 'lora_down': bd, 'lora_up': bu, 'lora_seg': kp}
+                self.wb[self._bwd_key(m)] = {'N': kp, 'K': N, 'bias': None, 'lora_down': bd, 'lora_up': bu,
+                                             'lora_seg': kp}
             rows.append([D.data_ptr(), U.data_ptr(), K, N, fdown, fup, bdown, bup])
         self._lora_keep = keep
         self.lora_table = torch.tensor(rows, dtype=torch.int64, device=self.dev)
-        self.refresh_lora()
+        self.load_lora_state_dict(lora)
 
     def refresh_lora(self):
         """Re-pack the flat LoRA parameters into the GEMM operand layouts (after load / optimiser step)."""
         ops.lora_pack(self.lora_table, self.lora_table.shape[0], self.lora_alpha)
 
+    def _up_perm(self, m):
+        """row permutation natural -> flat of module m's LoRA up (None = identity): the GEGLU projection's flat up is in the
+        packed row order of its GEMM"""
+        return geglu_perm(self.lora_views[m][5]).to(self.dev) if m.endswith(_GEGLU) else None
+
+    def load_lora_state_dict(self, lora):
+        """reference checkpoint tensors (down [r, K] or [r, K, 1, 1], up [N, r] or [N, r, 1, 1], rank r <= 4) -> the flat
+        state, then re-pack."""
+        for m, (D, U, _, _, K, N) in self.lora_views.items():
+            d = lora[f'{m}.lora_down.weight'].detach().to(self.dev, F32).reshape(-1, K)
+            u = lora[f'{m}.lora_up.weight'].detach().to(self.dev, F32).reshape(N, -1)
+            perm = self._up_perm(m)
+            if perm is not None:
+                u = u[perm]
+            D.zero_()
+            U.zero_()
+            D[:d.shape[0]] = d
+            U[:, :u.shape[1]] = u
+        self.refresh_lora()
+
+    def _natural(self, m, U):
+        perm = self._up_perm(m)
+        if perm is None:
+            return U.clone()
+        out = torch.empty_like(U)
+        out[perm] = U
+        return out
+
     def lora_state_dict(self):
-        """{f'{module}.lora_down.weight' [4,K], f'{module}.lora_up.weight' [N,4]} (trainer_edlora.py:371-378 keys)."""
+        """{f'{module}.lora_down.weight' [4,K], f'{module}.lora_up.weight' [N,4]} (trainer_edlora.py:371-378 keys); the 1x1
+        convs proj_in / proj_out as [4, K, 1, 1] / [N, 4, 1, 1] (the reference wraps a Conv2d there)."""
         out = {}
         for m, (D, U, _, _, _, _) in self.lora_views.items():
-            out[f'{m}.lora_down.weight'] = D.clone()
-            out[f'{m}.lora_up.weight'] = U.clone()
+            d, u = D.clone(), self._natural(m, U)
+            if m.endswith('.proj_in') or m.endswith('.proj_out'):
+                d, u = d[:, :, None, None], u[:, :, None, None]
+            out[f'{m}.lora_down.weight'] = d
+            out[f'{m}.lora_up.weight'] = u
         return out
 
     def lora_grad_dict(self):
-        return {m: (gD.clone(), gU.clone()) for m, (_, _, gD, gU, _, _) in self.lora_views.items()}
+        return {m: (gD.clone(), self._natural(m, gU)) for m, (_, _, gD, gU, _, _) in self.lora_views.items()}
 
     # ------------------------------------------------------------------------------------------ backward packs
     def _build_backward_packs(self):
@@ -173,23 +232,26 @@ class TrainEngine(UNetEngine):
             return {'W': Wb, 'N': cin, 'K': 9 * cout, 'bias': None}
 
         for key in list(self.w):
+            if key in self.wb:
+                continue            # a LoRA'd module's own pack (_build_lora_state): its weight is filled in below
             if key.endswith('.conv1') or key.endswith('.conv2') or key.endswith('upsamplers.0.conv'):
                 self.wb[key] = conv3(key)
             elif key.endswith('.conv_shortcut') or key.endswith('.proj_in') or key.endswith('.proj_out') or \
                     key.endswith('.ff1') or key.endswith('.ff2') or key.endswith('downsamplers.0.conv'):
                 self.wb[key] = lin(key)
         for m in self.lora_module_names():
-            if m not in self.wb:
+            bk = self._bwd_key(m)
+            if bk not in self.wb:
                 continue
             key, seg = self._fwd_slot(m)
             W = self.w[key]['W']
             N = self.lora_views[m][5]
             Wt = W[seg * N:(seg + 1) * N].t()
-            if self.wb[m]['N'] != Wt.shape[0]:                 # padded output width (text K / V: 768 -> 800)
-                Wp = torch.zeros(self.wb[m]['N'], N, device=self.dev, dtype=W.dtype)
+            if self.wb[bk]['N'] != Wt.shape[0]:                # padded output width (text K / V: 768 -> 800)
+                Wp = torch.zeros(self.wb[bk]['N'], N, device=self.dev, dtype=W.dtype)
                 Wp[:Wt.shape[0]] = Wt
                 Wt = Wp
-            self.wb[m]['W'] = Wt.contiguous()
+            self.wb[bk]['W'] = Wt.contiguous()
         self.d_ehs = None
         if self.text_grad:
             self.d_ehs = torch.zeros(len(self.xattn_names) * self.B * self.n_text, _r(self.cross_dim, 160), device=self.dev,
@@ -269,6 +331,11 @@ class TrainEngine(UNetEngine):
         ops.heads_transpose(Vc, Vct)
         return Kc, Vc, Kct, Vct
 
+    def _gemm_in(self, tn, tag, shape):
+        """input of proj_in / ff.net.0.proj / ff.net.2 / proj_out: kept for the LoRA gradient when those modules carry a
+        LoRA (`where: Transformer2DModel`), a scratch buffer otherwise"""
+        return self.tb(f'{tn}.{tag}', shape) if self.whole_block else self.buf('tr_' + tag, shape)
+
     def transformer_train(self, tn, x, out, h, w, C, xidx):
         B, Hh = self.B, self.heads
         N = h * w
@@ -278,7 +345,7 @@ class TrainEngine(UNetEngine):
         dp, dv = _r(d, 64), _r(d, 16)
         tbn = tn + '.transformer_blocks.0'
         S = {}
-        gn = self.buf('tr_gn', (M, C))
+        gn = self._gemm_in(tn, 'gn', (M, C))
         self.groupnorm(x, tn + '.norm', gn, HW=N, C=C, eps=1e-6, silu=False)
         t0 = self.tb(tn + '.t0', (M, C))
         self.gemm(gn, self.w[tn + '.proj_in'], t0, M=M)
@@ -311,17 +378,17 @@ class TrainEngine(UNetEngine):
         t2 = self.tb(tn + '.t2', (M, C))
         self.gemm(ao2, self.w[tbn + '.attn2.out'], t2, M=M, residual=t1)
         # --- feed-forward (un-fused GEGLU: the pre-activation is kept for backward)
-        ln3 = self.buf('tr_ln', (M, C))
+        ln3 = self._gemm_in(tn, 'ln', (M, C))
         self.layernorm(t2, tbn + '.norm3', ln3, M=M, C=C)
         z = self.tb(tn + '.z', (M, 8 * C))
         self.gemm(ln3, self.w[tbn + '.ff1'], z, M=M)
-        ff = self.buf('tr_ff', (M, 4 * C))
+        ff = self._gemm_in(tn, 'ff', (M, 4 * C))
         ops.geglu_fwd(z, ff, M=M, H=4 * C)
-        t3 = self.buf('tr_t3', (M, C))
+        t3 = self._gemm_in(tn, 't3', (M, C))
         self.gemm(ff, self.w[tbn + '.ff2'], t3, M=M, residual=t2)
         self.gemm(t3, self.w[tn + '.proj_out'], out, M=M, residual=x)
         S.update(t0=t0, ln1=ln1, Q=Q, K=K, V=V, ao1=ao1, lse1=lse1, t1=t1, ln2=ln2, Q2=Q2, ao2=ao2, lse2=lse2,
-                 pcols=pcols, t2=t2, z=z)
+                 pcols=pcols, t2=t2, z=z, gn=gn, ln3=ln3, ff=ff, t3=t3)
         self.trace.append(('transformer', tn, x, out, h, w, C, xidx, S))
         self.pcols_by_layer[xidx] = (pcols, N)
         return out
@@ -358,13 +425,20 @@ class TrainEngine(UNetEngine):
         dp = _r(d, 64)
         tbn = tn + '.transformer_blocks.0'
         a1, a2 = tbn + '.attn1.', tbn + '.attn2.'
-        # proj_out, feed-forward
+        whole = self.whole_block
+        # proj_out, feed-forward (with `where: Transformer2DModel` their dX packs carry the LoRA term)
+        if whole:
+            self._lora_grad(tn + '.proj_out', S['t3'], dOut, M, lddy=dOut.stride(0))
         d_t3 = self.buf('g_t3', (M, C))
         self.gemm(dOut, self.wb[tn + '.proj_out'], d_t3, M=M, lda=dOut.stride(0))
+        if whole:
+            self._lora_grad(tbn + '.ff.net.2', S['ff'], d_t3, M)
         d_y = self.buf('g_ff', (M, 4 * C))
         self.gemm(d_t3, self.wb[tbn + '.ff2'], d_y, M=M)
         d_z = self.buf('g_z', (M, 8 * C))
         ops.geglu_bwd(S['z'], d_y, d_z, M=M, H=4 * C)
+        if whole:           # d_z and the flat LoRA up are both in the packed (interleaved) row order
+            self._lora_grad(tbn + _GEGLU, S['ln3'], d_z, M)
         d_ln = self.buf('g_ln', (M, C))
         self.gemm(d_z, self.wb[tbn + '.ff1'], d_ln, M=M)
         d_t2 = self.buf('g_t2', (M, C))
@@ -402,6 +476,8 @@ class TrainEngine(UNetEngine):
             self.gemm(sl, self.wb[a1 + p], d_ln, M=M, lda=3 * C, residual=d_ln if s > 0 else None)
         d_t0 = self.buf('g_t0', (M, C))
         ops.layernorm_bwd(S['t0'], d_ln, self.w[tbn + '.norm1'][0], d_t0, M=M, C=C, add=d_t1)
+        if whole:
+            self._lora_grad(tn + '.proj_in', S['gn'], d_t0, M)
         d_gn = self.buf('g_gn', (M, C))
         self.gemm(d_t0, self.wb[tn + '.proj_in'], d_gn, M=M)
         g, b = self.w[tn + '.norm']

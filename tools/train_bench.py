@@ -3,6 +3,7 @@ synthetic data, random-init weights.  One process per GPU; the batch is sharded 
 ONLY collective is one NCCL all-reduce of the flat LoRA gradient (3.19 MB) per step.
 
   python tools/train_bench.py --batch 4                      # config 2 (1 GPU, batch 4)
+  python tools/train_bench.py --batch 4 --where Transformer2DModel   # LoRA on whole transformer blocks
   python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 tools/train_bench.py --batch 8   # config 5
 Timed region: K x (forward + loss + backward CUDA graph, all-reduce, AdamW + LoRA re-pack), CUDA events, max over ranks.
 """
@@ -23,6 +24,8 @@ def main():
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--no-reg', action='store_true')
+    ap.add_argument('--where', default='Attention', choices=('Attention', 'Transformer2DModel'),
+                    help='UNet LoRA placement (lora_cfg.where)')
     a = ap.parse_args()
     import torch.distributed as dist
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -36,8 +39,17 @@ def main():
     from mos_b200.train_engine import TrainEngine
     import bench
     sd, lora = bench.build_workload(False)[:2]
+    if a.where != 'Attention':          # the wider placement adds pairs for proj_in / proj_out / ff.net.0.proj / ff.net.2
+        from mixofshow.pipelines.trainer_edlora import _NameProbe
+        gl = torch.Generator().manual_seed(11)
+        for m in TrainEngine.lora_module_names.__get__(_NameProbe({}, a.where))():
+            if f'{m}.lora_down.weight' not in lora:
+                w = sd[m + '.weight']
+                n, k = w.shape[0], w[0].numel()
+                lora[f'{m}.lora_down.weight'] = (torch.rand(4, k, generator=gl) * 2 - 1) / k ** 0.5
+                lora[f'{m}.lora_up.weight'] = torch.randn(n, 4, generator=gl) * 0.02
     B = a.batch
-    eng = TrainEngine(sd, B, 64, 64, lora=lora, attn_reg_weight=None if a.no_reg else 0.01)
+    eng = TrainEngine(sd, B, 64, 64, lora=lora, attn_reg_weight=None if a.no_reg else 0.01, where=a.where)
     g = torch.Generator().manual_seed(100 + rank)
     x0 = torch.randn(B, 4, 64, 64, generator=g).cuda()
     noise = torch.randn(B, 4, 64, 64, generator=g).cuda()
@@ -76,7 +88,7 @@ def main():
                           'ms_per_step': round(ms, 3), 'batch_per_gpu': B, 'global_batch': B * world,
                           'scaling': 'weak', 'allreduce_bytes_per_step': (eng.state.n + 2) * 4,
                           'lora_params': eng.state.n, 'loss': round(loss, 5), 'data': 'synthetic',
-                          'attn_reg': not a.no_reg}))
+                          'attn_reg': not a.no_reg, 'where': a.where}))
     if world > 1:
         dist.destroy_process_group()
 
