@@ -5,9 +5,11 @@
 // Persistent kernel: one CTA per SM loops over 128 x 160 output tiles (160 divides every SD1.5 channel count).
 // Roles (256 + 32 threads):
 //   warps 0..7  two consumer warpgroups, 64 tile rows each: wgmma m64n160k16 (A and W from shared memory), then the fused
-//               epilogue straight from the accumulator registers
+//               epilogue from the accumulator registers into the staging tile (16-bit row output)
 //   warp 8      TMA producer   cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx; it runs ahead into
-//               the next tile while the consumers are in their epilogue
+//               the next tile while the consumers are in their epilogue.  16-bit row output: after a tile's last k block
+//               it loads the tile's residual into the staging tile, and once the consumers have filled the staging tile
+//               it writes it out with TMA stores (rows past M / H / B are clipped by the tensor map bounds).
 // LoRA fusion (edlora.py:244-246): the rank-padded down matrix [16, K] rides along as 16 extra W rows of the stage, and a
 // second wgmma (m64n16k16) on the same A descriptor produces t = x * down^T; the epilogue adds t * (alpha*up)^T.
 // Convolution: the A tile is a TW x TH x TB pixel patch of the NHWC activation fetched by a 4-D tensor map at
@@ -29,7 +31,12 @@ constexpr int B_STAGE_BYTES = BN * BK * 2;               // 20480
 constexpr int CONSUMER_THREADS = 256;                    // two warpgroups
 constexpr int NUM_THREADS = CONSUMER_THREADS + 32;       // + the TMA producer warp
 constexpr int PRODUCER_WARP = CONSUMER_THREADS / 32;
-constexpr int MAX_DYN_SMEM = 227 * 1024 - 2048;  // leave room for the static barriers
+constexpr int MAX_DYN_SMEM = 227 * 1024 - 6144;  // leave room for the static epilogue operands and barriers
+constexpr int EPI_BATCHES = 5;   // batches one 128-row tile can span (plain: rows_per_batch >= 32; conv: TB <= 4)
+// Staging tile of the 16-bit row output: 5 column boxes of [128 rows][w columns], w = 32 (row output, SWIZZLE_64B) or
+// 16 (GEGLU's 80 output columns, SWIZZLE_32B), each box the smem image of one TMA store / residual load.
+constexpr int EPI_BYTES = BM * BN * 2;                   // 40960
+constexpr int EPI_BOXES = 5;
 
 struct GemmDev {
   int M, N;
@@ -58,6 +65,10 @@ struct GemmDev {
   int heads, head_dim, dpad, dv_pad;
   long long tokens_per_batch;
   int accum;           // MOS_OUT_F32: out += result (Gram accumulation)
+  int epi_tma;         // 16-bit row output TMA can address: staged epilogue written by TMA stores (tensor map tmO)
+  int res_tma;         // epi_tma and the residual is prefetched into the staging tile by TMA (tensor map tmR)
+  int epi_lgw;         // log2 of the staging box width in columns (5: row output, 4: GEGLU)
+  int epi_copy;        // other 16-bit output (head-split, unaligned rows): staged epilogue, copied out by the consumers
   unsigned long long* tl;   // optional timeline buffer (mos_debug_set_timeline)
   int* counters;       // split-K with in-kernel finalize: one arrival counter per output tile (zero between launches)
   const uint8_t* pf;   // optional: bytes to pull into L2 for a LATER launch (the next layer's weights), see mos_gemm_args
@@ -114,6 +125,45 @@ __device__ __forceinline__ bool row_coord(const GemmDev& p, const TileCoord& t, 
   return m < p.M;
 }
 
+// Byte offset of (tile row r, output column c) in the staging tile: box c / w, rows of 2w bytes, the 16-byte chunk index
+// XOR-ed with address bits [7, 7 + log2(w/8)) of the row, which is the TMA SWIZZLE_32B / SWIZZLE_64B pattern.  A warp's
+// store of one fragment column pair (8 rows x 16 bytes) then touches 32 distinct banks.
+__device__ __forceinline__ uint32_t epi_off(int r, int c, int lgw) {
+  const int cin = c & ((1 << lgw) - 1);
+  const int chunk = (cin >> 3) ^ ((r >> (6 - lgw)) & ((1 << (lgw - 3)) - 1));
+  return ((c >> lgw) << (lgw + 8)) + (r << (lgw + 1)) + (chunk << 4) + ((cin & 7) << 1);
+}
+
+// Copy-out staging layout (head-split output, and row output whose destination TMA cannot address): 20 regions of 2 KB,
+// one per 8-column group.  Row-major groups hold row r's 8 columns at r * 16; transposed groups (V^T columns) hold
+// column c's 128 rows as 16 chunks of 8 rows, chunk index XOR-ed with c % 8, so that both the fragment writes and the
+// 16-byte chunk reads of a warp touch distinct banks.
+__device__ __forceinline__ uint32_t cp_off(int r, int c, bool tr) {
+  const int k = c >> 3, cc = c & 7;
+  return tr ? (k << 11) + (cc << 8) + ((((r >> 3) ^ cc) & 15) << 4) + ((r & 7) << 1) : (k << 11) + (r << 4) + (cc << 1);
+}
+// head-split output: global column nc belongs to a V^T segment
+__device__ __forceinline__ bool col_transposed(const GemmDev& p, int nc) {
+  return p.out_mode == MOS_OUT_HEADS && p.seg_kind[nc / (p.heads * p.head_dim)] == MOS_SEG_TRANSPOSED;
+}
+// destination of the 16-bit output element (row m, tile column c) of the tile at t
+__device__ __forceinline__ uint16_t* out_elem(const GemmDev& p, const TileCoord& t, long long m, int c) {
+  if (p.out_mode != MOS_OUT_HEADS)
+    return reinterpret_cast<uint16_t*>(p.out) + m * p.ldc + (p.geglu ? t.n0 / 2 : t.n0) + c;
+  const int nc = t.n0 + c;
+  const int seg_len = p.heads * p.head_dim;
+  const long long bb = m / p.tokens_per_batch;
+  const long long tok = m - bb * p.tokens_per_batch;
+  const int seg = nc / seg_len;
+  const int cc2 = nc - seg * seg_len;
+  const int head = cc2 / p.head_dim;
+  const int j = cc2 - head * p.head_dim;
+  uint16_t* base = reinterpret_cast<uint16_t*>(p.seg_ptr[seg]);
+  const long long bh = bb * p.heads + head;
+  if (p.seg_kind[seg] == MOS_SEG_ROWS) return base + (bh * p.seg_rows_pad[seg] + tok) * p.dpad + j;
+  return base + (bh * p.dv_pad + j) * p.seg_rows_pad[seg] + tok;
+}
+
 // bias (+ per-batch bias) of output column n for a row of batch b
 __device__ __forceinline__ float col_bias(const GemmDev& p, int b, int n) {
   float v = p.bias ? __ldg(p.bias + n) : 0.f;
@@ -133,11 +183,8 @@ __device__ __forceinline__ float4 lora_ranks(const float (&lacc)[LORA_N / 2], in
   return make_float4(__shfl_sync(quad, v0, s, 4), __shfl_sync(quad, v1, s, 4), __shfl_sync(quad, v0, s + 1, 4),
                      __shfl_sync(quad, v1, s + 1, 4));
 }
-// LoRA term of output column n: t[4 ranks of n's segment] . (alpha * up)[n]
-__device__ __forceinline__ float lora_term(const GemmDev& p, float4 t, int n) {
-  const float4 u = __ldg(reinterpret_cast<const float4*>(p.lora_up) + n);
-  return t.x * u.x + t.y * u.y + t.z * u.z + t.w * u.w;
-}
+// LoRA term of an output column: t[4 ranks of the column's segment] . (alpha * up)[column]
+__device__ __forceinline__ float lora_term(float4 t, float4 u) { return t.x * u.x + t.y * u.y + t.z * u.z + t.w * u.w; }
 
 // F16: 16-bit type of A, of the row / head-split outputs and of the residual (fp16 or bf16).
 // LORA: the fused LoRA branch is present (a template parameter, so that the k16 wgmma chain of a k block is straight-line
@@ -145,14 +192,23 @@ __device__ __forceinline__ float lora_term(const GemmDev& p, float4 t, int n) {
 template <bool F16, bool LORA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmL, const GemmDev p) {
+            const __grid_constant__ CUtensorMap tmL, const __grid_constant__ CUtensorMap tmO,
+            const __grid_constant__ CUtensorMap tmR, const GemmDev p) {
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment is required by SWIZZLE_128B
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte alignment is required by SWIZZLE_128B (an offset from smem_raw, so that the compiler keeps the pointer in
+  // the shared address space: the epilogue's staging stores then cannot alias global memory)
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   constexpr int stage_bytes = A_STAGE_BYTES + (LORA ? BN + LORA_N : BN) * 128;
+  uint8_t* epi = smem + p.stages * stage_bytes;            // staging tile (p.epi_tma), 1024-byte aligned
 
   __shared__ uint64_t full_bar[MAX_STAGES];
   __shared__ uint64_t empty_bar[MAX_STAGES];
+  __shared__ uint64_t epi_ready;   // producer -> consumers: the staging tile is free (and holds the tile's residual)
+  __shared__ uint64_t epi_full;    // consumers -> producer: the staging tile holds the finished output tile
+  // the tile's epilogue operands, loaded before its first store: bias + per-batch bias of the batches the tile spans
+  // (col_bias), and the LoRA up rows (alpha * up)
+  __shared__ float s_bias[EPI_BATCHES][BN];
+  __shared__ float4 s_lup[LORA ? BN : 1];
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -162,10 +218,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (LORA) tma_prefetch_desc(&tmL);
+    if (p.epi_tma) {
+      tma_prefetch_desc(&tmO);
+      if (p.res_tma) tma_prefetch_desc(&tmR);
+    }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);                          // one arrive.expect_tx by the producer
       mbar_init(&empty_bar[s], CONSUMER_THREADS / 32);     // one arrival per consumer warp
     }
+    mbar_init(&epi_ready, 1);
+    mbar_init(&epi_full, CONSUMER_THREADS);
     fence_barrier_init();
   }
   __syncthreads();
@@ -190,9 +252,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // ===================================================================== TMA producer
     if (lane == 0) {
       stamp(2);
+      const int box_w = 1 << p.epi_lgw;
+      // staging box j of the tile at t (output column c0 + j w); conv tiles are TW x TH x TB pixel boxes
+      auto epi_box = [&](const TileCoord& t, int c0, int j, auto&& op) {
+        if (p.conv) op(epi + (j << (p.epi_lgw + 8)), c0 + j * box_w, t.cw0, t.ch0, t.cb0);
+        else op(epi + (j << (p.epi_lgw + 8)), c0 + j * box_w, t.m0, 0, 0);
+      };
+      // write out item i (tile t) once the consumers have staged it; returns when the staging tile may be reused
+      auto epi_store = [&](const TileCoord& t, int i) {
+        mbar_wait_hint(&epi_full, i & 1);
+        const int c0 = p.geglu ? t.n0 / 2 : t.n0;
+        for (int j = 0; j < EPI_BOXES; ++j)
+          epi_box(t, c0, j, [&](const uint8_t* s, int x, int y, int z, int w) {
+            if (p.conv) tma_store_4d(&tmO, s, x, y, z, w);
+            else tma_store_2d(&tmO, s, x, y);
+          });
+        bulk_commit();
+        bulk_wait_read_all();
+        if (i == 0) stamp(5);
+      };
       int stage = 0;
       uint32_t phase = 0;
-      for (int ws = blockIdx.x; ws < p.total_items; ws += gridDim.x) {
+      int it = 0;
+      TileCoord prev{};
+      for (int ws = blockIdx.x; ws < p.total_items; ws += gridDim.x, ++it) {
         const TileCoord t = item_coord(p, ws);
         const int kb_begin = t.split * p.kb_per_split;
         const int kb_end = min(p.kb_total, kb_begin + p.kb_per_split);
@@ -216,6 +299,27 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             phase ^= 1;
           }
         }
+        if (p.epi_tma) {
+          // the previous item's output leaves the staging tile, then this item's residual lands in it.  The producer is
+          // here once it has issued this item's last k block: in a CTA with one item that is early in the consumers'
+          // mainloop; with several items, the previous item's write-out waits until here, and with it this residual.
+          if (it > 0) epi_store(prev, it - 1);
+          if (p.res_tma) {
+            mbar_expect_tx(&epi_ready, (uint32_t)EPI_BYTES);   // out-of-bounds box elements count too (zero fill)
+            for (int j = 0; j < EPI_BOXES; ++j)
+              epi_box(t, t.n0, j, [&](uint8_t* s, int x, int y, int z, int w) {
+                if (p.conv) tma_load_4d(s, &tmR, &epi_ready, x, y, z, w);
+                else tma_load_2d(s, &tmR, &epi_ready, x, y);
+              });
+          } else {
+            mbar_arrive(&epi_ready);
+          }
+          prev = t;
+        }
+      }
+      if (p.epi_tma && it > 0) {
+        epi_store(prev, it - 1);
+        bulk_wait_all();                                   // the global writes complete before the CTA exits
       }
     }
   } else {
@@ -278,13 +382,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
       if (et == 0 && it == 0) stamp(4);
-      // ---- epilogue, straight from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e)
+      int b_lo;                                            // batch of the tile's first row (s_bias slot 0)
+      {
+        long long m0;
+        row_coord(p, t, 0, m0, b_lo);
+      }
+      if (p.splits == 1) {                                 // (split-K partial tiles take no epilogue operands)
+        epi_bar();                // every consumer is done with the previous tile's operands and its copy-out reads
+        for (int i = et; i < EPI_BATCHES * BN; i += CONSUMER_THREADS) {
+          const int j = i / BN, c = i - j * BN;
+          s_bias[j][c] = b_lo + j < p.nbatch ? col_bias(p, b_lo + j, t.n0 + c) : 0.f;
+        }
+        if constexpr (LORA)
+          if (et < BN) s_lup[et] = __ldg(reinterpret_cast<const float4*>(p.lora_up) + t.n0 + et);
+        epi_bar();
+      }
+      // ---- epilogue from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e).  16-bit
+      // output (rows, GEGLU, head-split) goes to the staging tile; only fp32 output and split-K partials go to global.
+      if (p.epi_tma) mbar_wait(&epi_ready, it & 1);
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int r = rA + 8 * hr;
         long long m;
         int b;
         if (!row_coord(p, t, r, m, b)) continue;
+        const int bs = p.bias_batch ? b - b_lo : 0;     // s_bias slot of the row
         if (!LORA && p.splits > 1) {               // (the host rejects LoRA together with split-K)
           float* dst = p.partial + ((long long)t.split * p.M + m) * p.N + t.n0 + cq;
 #pragma unroll
@@ -292,7 +414,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
         } else if (p.geglu) {
           // tile columns [0,80) = a, [80,160) = gate for the same 80 outputs (columns n0/2 + [0,80) of the output)
-          __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(p.out) + m * p.ldc + t.n0 / 2;
           float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f);
           if constexpr (LORA) t0 = lora_ranks(lacc, hr, 0, lane);
 #pragma unroll
@@ -301,15 +422,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             float o[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              float a = acc[4 * i + 2 * hr + e] + col_bias(p, b, t.n0 + na + e);
-              float g = acc[4 * (i + BN / 16) + 2 * hr + e] + col_bias(p, b, t.n0 + ng + e);
+              float a = acc[4 * i + 2 * hr + e] + s_bias[bs][na + e];
+              float g = acc[4 * (i + BN / 16) + 2 * hr + e] + s_bias[bs][ng + e];
               if constexpr (LORA) {
-                a += lora_term(p, t0, t.n0 + na + e);
-                g += lora_term(p, t0, t.n0 + ng + e);
+                a += lora_term(t0, s_lup[na + e]);
+                g += lora_term(t0, s_lup[ng + e]);
               }
               o[e] = a * gelu_erf(g);
             }
-            *reinterpret_cast<uint32_t*>(orow + na) = pack16x2<F16>(o[0], o[1]);
+            *reinterpret_cast<uint32_t*>(epi + (p.epi_tma ? epi_off(r, na, p.epi_lgw) : cp_off(r, na, false))) =
+                pack16x2<F16>(o[0], o[1]);
           }
         } else {
           int seg = -1;                             // LoRA segment whose rank values are in tt
@@ -319,7 +441,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const int nc = t.n0 + 8 * i + cq;       // global column of the pair (nc, nc + 1)
             float o[2];
 #pragma unroll
-            for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + col_bias(p, b, nc + e);
+            for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + s_bias[bs][8 * i + cq + e];
             if constexpr (LORA) {
               // segments are multiples of 16 columns wide: seg is the same for the whole 8-column group, so uniform
               // over the warp, and it changes at most 3 times along the tile
@@ -329,17 +451,27 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 tt = lora_ranks(lacc, hr, sg, lane);
               }
 #pragma unroll
-              for (int e = 0; e < 2; ++e) o[e] += lora_term(p, tt, nc + e);
+              for (int e = 0; e < 2; ++e) o[e] += lora_term(tt, s_lup[8 * i + cq + e]);
             }
-            if (p.out_mode == MOS_OUT_BF16) {
-              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + m * p.ldc + nc;
-              if (p.residual) {
-                const float2 f = unpack16x2<F16>(*reinterpret_cast<const uint32_t*>(p.residual + m * p.ldr + nc));
+            const int cl = 8 * i + cq;              // tile column of the pair
+            if (p.out_mode != MOS_OUT_F32) {
+              if (p.residual) {                     // (row output only: the host drops it for head-split output)
+                const float2 f = unpack16x2<F16>(
+                    p.res_tma ? *reinterpret_cast<const uint32_t*>(epi + epi_off(r, cl, p.epi_lgw))
+                              : *reinterpret_cast<const uint32_t*>(p.residual + m * p.ldr + nc));
                 o[0] += f.x;
                 o[1] += f.y;
               }
-              *reinterpret_cast<uint32_t*>(dst) = pack16x2<F16>(o[0], o[1]);
-            } else if (p.out_mode == MOS_OUT_F32) {
+              const uint32_t v = pack16x2<F16>(o[0], o[1]);
+              if (p.epi_tma) {
+                *reinterpret_cast<uint32_t*>(epi + epi_off(r, cl, p.epi_lgw)) = v;
+              } else if (!col_transposed(p, nc)) {
+                *reinterpret_cast<uint32_t*>(epi + cp_off(r, cl, false)) = v;
+              } else {
+                *reinterpret_cast<uint16_t*>(epi + cp_off(r, cl, true)) = (uint16_t)(v & 0xFFFFu);
+                *reinterpret_cast<uint16_t*>(epi + cp_off(r, cl + 1, true)) = (uint16_t)(v >> 16);
+              }
+            } else {
               float2* dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nc);
               float2 r2 = make_float2(o[0], o[1]);
               if (p.accum) {
@@ -348,29 +480,50 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 r2.y += old.y;
               }
               *dst = r2;
-            } else {  // MOS_OUT_HEADS (head_dim % 8 == 0: both columns of the pair are in one head)
-              const int seg_len = p.heads * p.head_dim;
-              const long long bb = m / p.tokens_per_batch;
-              const long long tok = m - bb * p.tokens_per_batch;
-              const int seg = nc / seg_len;
-              const int cc2 = nc - seg * seg_len;
-              const int head = cc2 / p.head_dim;
-              const int j0 = cc2 - head * p.head_dim;
-              __nv_bfloat16* base = reinterpret_cast<__nv_bfloat16*>(p.seg_ptr[seg]);
-              const long long bh = bb * p.heads + head;
-              if (p.seg_kind[seg] == MOS_SEG_ROWS) {
-                *reinterpret_cast<uint32_t*>(base + (bh * p.seg_rows_pad[seg] + tok) * p.dpad + j0) =
-                    pack16x2<F16>(o[0], o[1]);
-              } else {
-                uint16_t* d = reinterpret_cast<uint16_t*>(base + (bh * p.dv_pad + j0) * p.seg_rows_pad[seg] + tok);
-                d[0] = cvt16<F16>(o[0]);
-                d[p.seg_rows_pad[seg]] = cvt16<F16>(o[1]);
-              }
             }
           }
         }
       }
-      if (et == 0 && it == 0) stamp(5);
+      if (p.epi_tma) {
+        fence_proxy_async_smem();                          // this thread's staging writes -> the TMA store's reads
+        mbar_arrive(&epi_full);
+      } else {
+        if (p.epi_copy) {
+          // ---- copy-out: 16-byte chunks of the staging tile (8 columns of a row, or 8 rows of a V^T column) to their
+          // destination, one 16-byte store where the 8 elements are contiguous and aligned there.  The rest (V^T
+          // tokens across a batch boundary at a token count that is not a multiple of 8, unaligned row output) is
+          // written element by element from the same chunk.
+          epi_bar();
+          const int groups = (p.geglu ? BN / 2 : BN) / 8;
+          for (int idx = et; idx < groups * BM; idx += CONSUMER_THREADS) {
+            const int k = idx / BM, rs = idx % BM;
+            const bool tr = col_transposed(p, t.n0 + 8 * k);
+            const int r0 = tr ? (rs & ~7) : rs;           // V^T: 8 rows of column 8k + rs % 8
+            const int c0 = tr ? 8 * k + (rs & 7) : 8 * k;
+            const uint8_t* src = epi + cp_off(r0, c0, tr);
+            long long m0, m7;
+            int bq;
+            uint16_t* d0 = nullptr;
+            bool vec = row_coord(p, t, r0, m0, bq);
+            if (vec) {
+              d0 = out_elem(p, t, m0, c0);
+              vec = (reinterpret_cast<uintptr_t>(d0) & 15) == 0;
+              if (tr) vec = vec && row_coord(p, t, r0 + 7, m7, bq) && out_elem(p, t, m7, c0) == d0 + 7;
+            }
+            if (vec) {
+              *reinterpret_cast<uint4*>(d0) = *reinterpret_cast<const uint4*>(src);
+            } else {
+#pragma unroll 1
+              for (int e = 0; e < 8; ++e) {
+                long long me;
+                if (row_coord(p, t, tr ? r0 + e : r0, me, bq))
+                  *out_elem(p, t, me, tr ? c0 : c0 + e) = *reinterpret_cast<const uint16_t*>(src + 2 * e);
+              }
+            }
+          }
+        }
+        if (et == 0 && it == 0) stamp(5);
+      }
       if (!LORA && p.counters != nullptr) {
         // split-K, in-kernel finalize: publish this item's partial tile (bar.sync ordered every consumer thread's stores
         // before this thread; its gpu-scope fence is cumulative over them - the pattern of a cooperative grid sync)
@@ -562,8 +715,10 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
 
   GemmDev p;
   memset(&p, 0, sizeof(p));
-  CUtensorMap tmA, tmB, tmL;
+  CUtensorMap tmA, tmB, tmL, tmO, tmR;
   memset(&tmL, 0, sizeof(tmL));
+  memset(&tmO, 0, sizeof(tmO));
+  memset(&tmR, 0, sizeof(tmR));
   p.M = (int)a->M;
   p.N = (int)a->N;
   p.conv = a->conv;
@@ -668,6 +823,42 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   p.dv_pad = a->dv_pad;
   p.tokens_per_batch = a->tokens_per_batch > 0 ? a->tokens_per_batch : 1;
   p.accum = a->accumulate;
+  // Every 16-bit output goes through the staging tile.  Row output (with GEGLU and residual) that TMA can address (16-byte
+  // aligned base, row pitch a multiple of 8 elements) is written by TMA stores, its residual prefetched by TMA when that
+  // is addressable too: tensor maps with the tile's row geometry (plain [M, cols], conv [B, H, W, cols]), one box per
+  // staging box.  Head-split output and other row output are copied out of the staging tile by the consumers.
+  const uint64_t cols = (uint64_t)(a->geglu ? a->N / 2 : a->N);
+  auto tma_rows = [&](const void* base, long long ld) {
+    return base != nullptr && ld >= (long long)cols && ld % 8 == 0 && is_aligned(base, 16);
+  };
+  if (a->geglu || a->out_mode == MOS_OUT_HEADS) p.residual = nullptr;   // neither takes a residual
+  p.epi_tma = (a->out_mode == MOS_OUT_BF16 && splits == 1 && tma_rows(a->out, a->ldc)) ? 1 : 0;
+  p.res_tma = (p.epi_tma && p.residual != nullptr && tma_rows(a->residual, a->ldr)) ? 1 : 0;
+  p.epi_copy = (a->out_mode != MOS_OUT_F32 && splits == 1 && !p.epi_tma) ? 1 : 0;
+  if (p.epi_tma) {
+    p.epi_lgw = a->geglu ? 4 : 5;
+    const uint32_t bw = 1u << p.epi_lgw;
+    const int swz = a->geglu ? 1 : 2;        // SWIZZLE_32B / SWIZZLE_64B: rows of 2 bw bytes (epi_off)
+    auto row_map = [&](CUtensorMap* tm, const void* base, long long ld) -> int {
+      const uint64_t pitch = (uint64_t)ld * 2;
+      if (a->conv) {
+        uint64_t dims[4] = {cols, (uint64_t)a->Wd, (uint64_t)a->H, (uint64_t)a->B};
+        uint64_t str[3] = {pitch, (uint64_t)a->Wd * pitch, (uint64_t)a->H * a->Wd * pitch};
+        uint32_t box[4] = {bw, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TB};
+        return encode_tmap(tm, base, 2, 4, dims, str, box, swz);
+      }
+      uint64_t dims[2] = {cols, (uint64_t)a->M};
+      uint64_t str[1] = {pitch};
+      uint32_t box[2] = {bw, (uint32_t)BM};
+      return encode_tmap(tm, base, 2, 2, dims, str, box, swz);
+    };
+    int rc = row_map(&tmO, a->out, a->ldc);
+    if (rc) return rc;
+    if (p.res_tma) {
+      rc = row_map(&tmR, a->residual, a->ldr);
+      if (rc) return rc;
+    }
+  }
   p.tl = g_timeline_host;
   p.pf = nullptr;
   p.pf_bytes = 0;
@@ -701,10 +892,11 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   const int stage_bytes = A_STAGE_BYTES + (lora ? BN + LORA_N : BN) * 128;
   int stages = a->stages > 0 ? a->stages : (stages_env > 0 ? stages_env : MAX_STAGES);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
-  while (stages * stage_bytes + 1024 > MAX_DYN_SMEM) --stages;
+  const int epi_bytes = (p.epi_tma || p.epi_copy) ? EPI_BYTES : 0;
+  while (stages * stage_bytes + epi_bytes + 1024 > MAX_DYN_SMEM) --stages;
   if (stages < 2) stages = 2;
   p.stages = stages;
-  const int smem_bytes = stages * stage_bytes + 1024;
+  const int smem_bytes = stages * stage_bytes + epi_bytes + 1024;
 
   static bool configured = false;
   if (!configured) {
@@ -718,7 +910,7 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   const int units = p.total_items < num_sms ? p.total_items : num_sms;
   auto kern = f16 ? (lora ? gemm_kernel<true, true> : gemm_kernel<true, false>)
                   : (lora ? gemm_kernel<false, true> : gemm_kernel<false, false>);
-  MOS_CHECK_CUDA(launch_pdl(kern, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA, tmB, tmL, p));
+  MOS_CHECK_CUDA(launch_pdl(kern, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA, tmB, tmL, tmO, tmR, p));
   return MOS_OK;
 }
 
