@@ -413,26 +413,49 @@ def merge_kv_in_cross_attention(unet_state_dict, cross_kv_layer_names, text_feat
 
 class _RowRecorder:
     """CLIPTextEngine hook for the text-encoder fusion: keeps the rows of the valid (un-padded) token positions of
-    every recorded GEMM input as fp32 (a few hundred rows of 768: no tensor-core Gram needed)."""
+    every recorded GEMM input as fp32 (a few hundred rows of 768 / 3072: no tensor-core Gram needed).
+    keys: the record keys some solve uses (None: all)."""
 
-    def __init__(self, rows, heads, d, dh):
-        self.rows, self.heads, self.d, self.dh = rows, heads, d, dh
+    def __init__(self, rows, heads, d, dh, keys=None):
+        self.rows, self.heads, self.d, self.dh, self.keys = rows, heads, d, dh, keys
         self.X = {}
 
     def __call__(self, key, A, M, C):
+        if self.keys is not None and key not in self.keys:
+            return
         X = A[self.rows].float()
         if C == self.heads * self.dh and self.dh != self.d:       # attention output in the padded head layout
             X = X.view(-1, self.heads, self.dh)[:, :, :self.d].reshape(-1, self.heads * self.d)
         self.X[key] = X.contiguous()
 
 
-TEXT_KEYS = {'q_proj': 'self_attn.in', 'k_proj': 'self_attn.in', 'v_proj': 'self_attn.in', 'out_proj': 'self_attn.out_proj'}
+# module suffix of a fused weight -> suffix of the engine record key of its input (q|k|v share one input).  UNet keys are
+# relative to the Transformer2DModel ('...attentions.{j}': proj_in / proj_out) or its transformer_blocks.0 (the rest);
+# CLIP keys to 'text_model.encoder.layers.{i}'.  attn2.to_k / to_v read the text embeddings: merge_kv_in_cross_attention.
+RECORD_KEYS = (('.attn1.to_q', '.attn1.in'), ('.attn1.to_k', '.attn1.in'), ('.attn1.to_v', '.attn1.in'),
+               ('.attn1.to_out.0', '.attn1.to_out.0'), ('.attn2.to_q', '.attn2.to_q'),
+               ('.attn2.to_out.0', '.attn2.to_out.0'), ('.ff.net.0.proj', '.ff.net.0.proj'), ('.ff.net.2', '.ff.net.2'),
+               ('.proj_in', '.proj_in'), ('.proj_out', '.proj_out'),
+               ('.self_attn.q_proj', '.self_attn.in'), ('.self_attn.k_proj', '.self_attn.in'),
+               ('.self_attn.v_proj', '.self_attn.in'), ('.self_attn.out_proj', '.self_attn.out_proj'),
+               ('.mlp.fc1', '.mlp.fc1'), ('.mlp.fc2', '.mlp.fc2'))
+
+
+def record_key(name):
+    """'<module>.weight' of a spatial UNet or a CLIP linear -> the key under which the engine records its input, e.g.
+    '...transformer_blocks.0.attn1.to_k.weight' -> '...transformer_blocks.0.attn1.in'."""
+    mod = name[:-len('.weight')] if name.endswith('.weight') else name
+    for leaf, key in RECORD_KEYS:
+        if mod.endswith(leaf):
+            return mod[:-len(leaf)] + key
+    raise KeyError(f'{name}: no recorded input for this layer in gradient fusion')
 
 
 def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, optimize_iters, device='cuda',
                        pad_id=49407):
     """Text-encoder fusion (gradient_fusion.py:460-565).  text_encoder_list[c]: concept c's CLIP LoRA
-    ({'text_model.encoder.layers.{i}.self_attn.{q,k,v,out}_proj.lora_{down,up}.weight'}); prompt_ids[c]: the un-padded
+    ({'text_model.encoder.layers.{i}.self_attn.{q,k,v,out}_proj.lora_{down,up}.weight'}, with `where: CLIPEncoderLayer`
+    also '...layers.{i}.mlp.fc{1,2}.lora_{down,up}.weight'); prompt_ids[c]: the un-padded
     token-id sequences of concept c's 32 layer-bound prompts ('photo of a <c>' and '<c>' x 16, :515-520; the tokenizer
     runs upstream).  For every concept its LoRA is merged (:505-512), the prompts run through the GPU CLIP engine and
     the inputs of the LoRA'd linears at ALL valid token positions are recorded (the reference's forward hooks, :146-167,
@@ -441,6 +464,7 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
     padded to 77 for the engine and only the valid rows are kept."""
     from mos_b200.clip_engine import CLIPTextEngine
     names = sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in text_encoder_list for k in t})
+    keys = {record_key(n) for n in names}
     feats = []
     for c, tuned in enumerate(text_encoder_list):
         seqs = [torch.as_tensor(p_).reshape(-1) for p_ in prompt_ids[c]]
@@ -452,15 +476,14 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
             assert 0 < q.numel() <= eng.T
             ids[s_, :q.numel()] = q
             rows += [s_ * eng.T + t for t in range(q.numel())]
-        rec = _RowRecorder(torch.tensor(rows, device=device), eng.heads, eng.d, eng.dh)
+        rec = _RowRecorder(torch.tensor(rows, device=device), eng.heads, eng.d, eng.dh, keys)
         eng.gram_rec = rec
         eng(ids)
         feats.append(rec.X)
     jobs = []
     for name in names:                                       # e.g. 'text_model.encoder.layers.0.self_attn.q_proj.weight'
         mod = name[:-len('.weight')]
-        layer, leaf = mod.rsplit('.self_attn.', 1)
-        rec_key = layer + '.' + TEXT_KEYS[leaf]
+        rec_key = record_key(name)
         W0 = text_state_dict[name].to(device, F32)
         d_in = W0.shape[1]
         G = torch.zeros(d_in, d_in, device=device)
@@ -485,12 +508,15 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
 class GramRecorder:
     """Engine-side replacement of the reference's forward hooks (gradient_fusion.py:146-167): instead of copying
     every (input, output - bias) pair to host RAM, accumulate G += X^T X per recorded GEMM input on the tensor
-    cores (transpose -> wgmma GEMM with fp32 accumulate output)."""
+    cores (transpose -> wgmma GEMM with fp32 accumulate output).  keys: the record keys some solve uses (None: all); an
+    attention-only fusion then issues no Gram launch for the feed-forward / proj_in / proj_out inputs (ff.net.2: 5120^2)."""
 
-    def __init__(self, device):
-        self.dev, self.G, self.rows, self._xt = device, {}, {}, {}
+    def __init__(self, device, keys=None):
+        self.dev, self.G, self.rows, self._xt, self.keys = device, {}, {}, {}, keys
 
     def __call__(self, key, A, M, C):
+        if self.keys is not None and key not in self.keys:
+            return
         G = self.G.get(key)
         first = G is None
         if first:
@@ -504,23 +530,23 @@ class GramRecorder:
         self.rows[key] += M
 
 
-SPATIAL_KEYS = (('attn1.to_q', 'attn1.in'), ('attn1.to_k', 'attn1.in'), ('attn1.to_v', 'attn1.in'),
-                ('attn1.to_out.0', 'attn1.to_out.0'), ('attn2.to_q', 'attn2.to_q'), ('attn2.to_out.0', 'attn2.to_out.0'))
-
-
 def merge_spatial_attention(unet_state_dict, unet_spatial_attn_list, alphas, concept_embeds, optimize_iters,
                             latent_hw=(64, 64), num_inference_steps=20, seed=0, device='cuda', block_out=None,
                             layers=None):
     """Spatial-attention fusion (gradient_fusion.py:627-747).  concept_embeds[c] = layer-wise prompt embeddings
     [1,16,77,768] of 'photo of a <concept c>' (CLIP runs upstream).  For every concept: merge its LoRA, run the
     20-step DPM-Solver++ sampling (batch 1, no CFG, all steps recorded, :579-624) on the engine with the Gram
-    recorder, then solve every LoRA'd layer from the accumulated Gram matrices."""
+    recorder, then solve every LoRA'd layer from the accumulated Gram matrices.  Besides the attention projections this
+    covers the `where: Transformer2DModel` layers (proj_in / proj_out as 1x1 convs, returned 4-D; ff.net.0.proj solved in
+    the state-dict row order, ff.net.2)."""
     from mos_b200.engine import UNetEngine, ehs_to_layer_major
     from mos_b200.scheduler import DPMSolverPP2M
     H, Wd = latent_hw
     kw = {}
     if block_out is not None:
         kw = dict(block_out=block_out, layers=layers)
+    names = sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in unet_spatial_attn_list for k in t})
+    keys = {record_key(n) for n in names}
     grams, merged_w = [], []
     eng = None
     prof = os.environ.get('MOS_FUSION_PROFILE') == '1'       # stage timing printout (tools/config_bench.py)
@@ -540,7 +566,7 @@ def merge_spatial_attention(unet_state_dict, unet_spatial_attn_list, alphas, con
                              use_graph=False, **kw)
         else:
             eng.set_merged_lora(tuned, alphas[c], state_dict=unet_state_dict)   # only the LoRA'd projections are re-packed
-        rec = GramRecorder(device)
+        rec = GramRecorder(device, keys)
         eng.gram_rec = rec
         nx = len(eng.xattn_names)
         sched = DPMSolverPP2M()
@@ -560,13 +586,10 @@ def merge_spatial_attention(unet_state_dict, unet_spatial_attn_list, alphas, con
         merged_w.append(tuned)
         eng.gram_rec = None
     mark('job assembly')
-    names = sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in unet_spatial_attn_list for k in t})
     jobs = []
     for name in names:                                          # e.g. '...attn1.to_q.weight'
         mod = name[:-len('.weight')]
-        tb, leaf = mod.rsplit('.attn', 1)
-        leaf = 'attn' + leaf
-        rec_key = tb + '.' + dict(SPATIAL_KEYS)[leaf]
+        rec_key = record_key(name)
         W0 = unet_state_dict[name].to(device, F32).reshape(unet_state_dict[name].shape[0], -1)
         d_in = W0.shape[1]
         G = torch.zeros(d_in, d_in, device=device)
@@ -603,22 +626,26 @@ TEMPLATE_SIMPLE = 'photo of a {}'                      # gradient_fusion.py:19
 NUM_CROSS_ATTENTION_LAYERS = 16
 
 
-_UNET_LORA_SUFFIXES = tuple(f'.{a}.{p}.lora_{d}.weight' for a in ('attn1', 'attn2')
-                            for p in ('to_q', 'to_k', 'to_v', 'to_out.0') for d in ('down', 'up'))
-_TEXT_LORA_SUFFIXES = tuple(f'.self_attn.{p}.lora_{d}.weight' for p in ('q_proj', 'k_proj', 'v_proj', 'out_proj')
+# the layers the fusion stages solve (the reference's candidate lists, gradient_fusion.py:482-488 / :637-645)
+_UNET_LORA_SUFFIXES = tuple(f'.{m}.lora_{d}.weight'
+                            for m in [f'{a}.{p}' for a in ('attn1', 'attn2') for p in ('to_q', 'to_k', 'to_v', 'to_out.0')]
+                            + ['ff.net.0.proj', 'ff.net.2', 'proj_in', 'proj_out'] for d in ('down', 'up'))
+_TEXT_LORA_SUFFIXES = tuple(f'.{m}.lora_{d}.weight' for m in ('self_attn.q_proj', 'self_attn.k_proj', 'self_attn.v_proj',
+                                                               'self_attn.out_proj', 'mlp.fc1', 'mlp.fc2')
                             for d in ('down', 'up'))
 
 
 def _check_lora_targets(params, path):
-    """The fusion stages cover the reference's default LoRA placement (`where: Attention` / `where: CLIPAttention`, every
-    shipped options/train/EDLoRA/*.yml).  Checkpoints that also tune CLIP's mlp.fc1/fc2 (`where: CLIPEncoderLayer`) or the
-    UNet's ff.net / proj_in / proj_out (`where: Transformer2DModel`) are refused HERE, before any stage has run, instead
-    of failing with a KeyError half way through the fusion."""
+    """The fusion stages cover the reference's LoRA placements: `where: Attention` / `Transformer2DModel` in the UNet
+    (attention projections, ff.net, proj_in / proj_out) and `where: CLIPAttention` / `CLIPEncoderLayer` in the text encoder
+    (self_attn projections, mlp.fc1 / fc2).  A LoRA anywhere else (e.g. on a resnet conv) is refused HERE, before any stage
+    has run, instead of failing with a KeyError half way through the fusion."""
     bad = [k for k in (params.get('unet') or {}) if not k.endswith(_UNET_LORA_SUFFIXES)]
     bad += [k for k in (params.get('text_encoder') or {}) if not k.endswith(_TEXT_LORA_SUFFIXES)]
     if bad:
-        raise ValueError(f'{path}: unsupported LoRA target(s) {bad[:3]}{" ..." if len(bad) > 3 else ""}: gradient fusion on '
-                         'the GPU path handles attention-projection LoRA (where: Attention / CLIPAttention) only')
+        raise ValueError(f'{path}: unsupported LoRA target(s) {bad[:3]}{" ..." if len(bad) > 3 else ""}: gradient fusion '
+                         'handles LoRA on the transformer blocks (where: Attention / Transformer2DModel) and the CLIP encoder '
+                         'layers (where: CLIPAttention / CLIPEncoderLayer) only')
 
 
 def parse_new_concepts(concept_cfg):

@@ -226,9 +226,13 @@ class CLIPTextEngine:
             x1 = self.buf(f'x1_{i & 1}', (M, Cp))
             self._gemm(ao, ent['out'], x1, M=M, residual=x)
             ops.layernorm(x1, ent['ln2'][0], ent['ln2'][1], ln, M=M, C=C, eps=self.eps, ldx=Cp, ldy=C)
+            if self.gram_rec is not None:
+                self.gram_rec(key + 'mlp.fc1', ln, M, C)
             h = self.buf('h', (M, self.Ip))
             self._gemm(ln, ent['fc1'], h, M=M)
             ops.quick_gelu(h, M=M, C=self.Ip)
+            if self.gram_rec is not None:
+                self.gram_rec(key + 'mlp.fc2', h[:, :self.I], M, self.I)     # the I real columns of the padded buffer
             x2 = self.buf(f'x2_{i & 1}', (M, Cp))
             self._gemm(h, ent['fc2'], x2, M=M, residual=x1)
             x = x2

@@ -428,6 +428,8 @@ class UNetEngine:
         tb = tn + '.transformer_blocks.0'
         gn = self.buf('tr_gn', (M, C))
         self.groupnorm(x, tn + '.norm', gn, HW=N, C=C, eps=1e-6, silu=False)
+        if self.gram_rec is not None:
+            self.gram_rec(tn + '.proj_in', gn, M, C)
         t0 = self.buf('tr_t0', (M, C))
         self.gemm(gn, self.w[tn + '.proj_in'], t0, M=M)
         ln = self.buf('tr_ln', (M, C))
@@ -473,10 +475,16 @@ class UNetEngine:
         self.gemm(ao, self.w[tb + '.attn2.out'], t2, M=M, residual=t1)
         # --- feed-forward (GEGLU fused in the first GEMM's epilogue)
         self.layernorm(t2, tb + '.norm3', ln, M=M, C=C)
+        if self.gram_rec is not None:
+            self.gram_rec(tb + '.ff.net.0.proj', ln, M, C)
         ff = self.buf('tr_ff', (M, 4 * C))
         self.gemm(ln, self.w[tb + '.ff1'], ff, M=M, geglu=True)
+        if self.gram_rec is not None:
+            self.gram_rec(tb + '.ff.net.2', ff, M, 4 * C)
         t3 = self.buf('tr_t3', (M, C))
         self.gemm(ff, self.w[tb + '.ff2'], t3, M=M, residual=t2)
+        if self.gram_rec is not None:
+            self.gram_rec(tn + '.proj_out', t3, M, C)
         self.gemm(t3, self.w[tn + '.proj_out'], out, M=M, residual=x)
         return out
 

@@ -1,10 +1,12 @@
 """BASELINE config 3 END TO END on one H100: `gradient_fusion.compose_concepts` (the entry point `python gradient_fusion.py`
 drives) on a synthetic SD1.5-size model directory and 5 synthetic ED-LoRA concept checkpoints in the reference's
-on-disk layout - load, token / embedding merge, text-encoder merge (48 CLIPAttention linears x 500 L-BFGS iterations),
-cross-attention K/V merge (32 x 500), spatial-attention merge (96 x 50, incl. the recorded UNet forwards), save and
-re-load of the fused model.  Prints one JSON line with the wall-clock seconds of every stage.
+on-disk layout - load, token / embedding merge, text-encoder merge (48 CLIPAttention linears x 500 L-BFGS iterations;
+72 with `--text-where CLIPEncoderLayer`), cross-attention K/V merge (32 x 500), spatial merge (96 x 50, incl. the recorded
+UNet forwards; 160 with `--unet-where Transformer2DModel`), save and re-load of the fused model.  Prints one JSON line with
+the wall-clock seconds of every stage and the card they were measured on.
 
     python tools/compose_bench.py [--concepts 5] [--textenc-iters 500] [--unet-iters 50] [--tiny]
+                                  [--unet-where {Attention,Transformer2DModel}] [--text-where {CLIPAttention,CLIPEncoderLayer}]
 """
 import argparse
 import json
@@ -63,12 +65,50 @@ class WordTokenizer:
         return SimpleNamespace(input_ids=rows[0] if single else rows)
 
 
+def _lora_pair(g, W, rank=4):
+    """random rank-4 pair for the weight W ([out, in], or a 1x1 conv [out, in, 1, 1]) in the trainer's checkpoint shapes:
+    down ~ kaiming-uniform(a=sqrt(5)), up ~ N(0, 0.02^2) (as bench.random_unet_lora)"""
+    cout, cin, tail = W.shape[0], W.shape[1], tuple(W.shape[2:])
+    down = ((torch.rand(rank, cin, generator=g) * 2 - 1) / cin ** 0.5).reshape(rank, cin, *tail)
+    up = (torch.randn(cout, rank, generator=g) * 0.02).reshape(cout, rank, *tail)
+    return down, up
+
+
+def whole_block_unet_lora(sd, cfg, seed):
+    """`where: Transformer2DModel`: the attention LoRA of bench.random_unet_lora plus proj_in / proj_out (1x1 convs, saved
+    4-D) and ff.net.0.proj / ff.net.2 of every transformer block"""
+    from mos_b200.engine import cross_attention_names
+    lora = bench.random_unet_lora(sd, cfg, seed=seed)
+    g = torch.Generator().manual_seed(1000 + seed)
+    names = cross_attention_names(cfg['block_out_channels'], cfg['layers_per_block']) if cfg else cross_attention_names()
+    for an in names:
+        tn = an[:-len('.transformer_blocks.0.attn2')]
+        for m in (f'{tn}.proj_in', f'{tn}.transformer_blocks.0.ff.net.0.proj', f'{tn}.transformer_blocks.0.ff.net.2',
+                  f'{tn}.proj_out'):
+            lora[m + '.lora_down.weight'], lora[m + '.lora_up.weight'] = _lora_pair(g, sd[m + '.weight'])
+    return lora
+
+
+def gpu_card():
+    """name and power limit of the GPU the stages run on (the power limit bounds the clocks under sustained load)"""
+    import subprocess
+    name = torch.cuda.get_device_name()
+    try:
+        limit = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader', '-i',
+                                str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        limit = ''
+    return {'name': name, 'power_limit': limit or 'unknown'}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--concepts', type=int, default=5)
     ap.add_argument('--textenc-iters', type=int, default=500)       # fuse.sh / gradient_fusion.py defaults
     ap.add_argument('--unet-iters', type=int, default=50)
     ap.add_argument('--tiny', action='store_true')
+    ap.add_argument('--unet-where', choices=('Attention', 'Transformer2DModel'), default='Attention')
+    ap.add_argument('--text-where', choices=('CLIPAttention', 'CLIPEncoderLayer'), default='CLIPAttention')
     a = ap.parse_args()
     import gradient_fusion as gf
     from mixofshow.models.unet_b200 import UNet2DConditionModel
@@ -77,7 +117,8 @@ def main():
     work = tempfile.mkdtemp(prefix='compose_bench_')
     out = {'config': f'gradient_fusion.compose_concepts, {a.concepts} synthetic ED-LoRAs, '
                      f'{"tiny" if a.tiny else "SD1.5-size"} UNet + 12-layer CLIP text encoder, 1xH100',
-           'textenc_iters': a.textenc_iters, 'unet_iters': a.unet_iters}
+           'textenc_iters': a.textenc_iters, 'unet_iters': a.unet_iters, 'unet_where': a.unet_where,
+           'text_where': a.text_where, 'gpu': gpu_card()}
     try:
         t0 = time.perf_counter()
         sd, _, _, _, cfg = bench.build_workload(a.tiny)
@@ -89,6 +130,7 @@ def main():
         clip = CLIPTextModel(CLIPTextConfig(vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
                                             num_attention_heads=12, max_position_embeddings=77, hidden_act='quick_gelu')).eval()
         clip.save_pretrained(os.path.join(base, 'text_encoder'))
+        csd = clip.state_dict()
         cfgs = []
         for c in range(a.concepts):
             g = torch.Generator().manual_seed(50 + c)
@@ -99,14 +141,22 @@ def main():
                     m = f'text_model.encoder.layers.{i}.self_attn.{pj}'
                     tlora[m + '.lora_down.weight'] = (torch.rand(4, 768, generator=g) * 2 - 1) / 768 ** 0.5
                     tlora[m + '.lora_up.weight'] = torch.randn(768, 4, generator=g) * 0.02
+            if a.text_where == 'CLIPEncoderLayer':
+                gm = torch.Generator().manual_seed(1050 + c)
+                for i in range(12):
+                    for fc in ('fc1', 'fc2'):
+                        m = f'text_model.encoder.layers.{i}.mlp.{fc}'
+                        tlora[m + '.lora_down.weight'], tlora[m + '.lora_up.weight'] = _lora_pair(gm, csd[m + '.weight'])
+            ulora = (whole_block_unet_lora(sd, cfg, seed=10 + c) if a.unet_where == 'Transformer2DModel'
+                     else bench.random_unet_lora(sd, cfg, seed=10 + c))
             params = {'new_concept_embedding': {w: torch.randn(16, 768, generator=g) * 0.02 for w in words},
-                      'text_encoder': tlora, 'unet': bench.random_unet_lora(sd, cfg, seed=10 + c)}
+                      'text_encoder': tlora, 'unet': ulora}
             path = os.path.join(work, f'concept{c}.pth')
             torch.save({'params': params}, path)
             cfgs.append({'lora_path': path, 'unet_alpha': 1.0, 'text_encoder_alpha': 1.0, 'concept_name': ' '.join(words)})
         cfg_path = os.path.join(work, 'concepts.json')
         json.dump(cfgs, open(cfg_path, 'w'))
-        del unet, clip
+        del unet, clip, csd
         out['setup_seconds'] = round(time.perf_counter() - t0, 2)
         stamps = []
 
@@ -133,6 +183,11 @@ def main():
         out['fused_reload_ok'] = bool(torch.isfinite(w).all())
         d0 = sd['down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight']
         out['example_crosskv_delta_rel'] = round(((w.float().cpu() - d0).norm() / d0.norm()).item(), 5)
+        if a.unet_where == 'Transformer2DModel':
+            k = 'mid_block.attentions.0.transformer_blocks.0.ff.net.2.weight'
+            w = fused.state_dict()[k].float().cpu()
+            out['example_ff2_delta_rel'] = round(((w - sd[k]).norm() / sd[k].norm()).item(), 5)
+            out['fused_reload_ok'] = out['fused_reload_ok'] and bool(torch.isfinite(w).all())
         out['data'] = 'synthetic (random-init weights, random LoRAs up ~ N(0, 0.02^2), whitespace tokenizer stub)'
     finally:
         shutil.rmtree(work, ignore_errors=True)
