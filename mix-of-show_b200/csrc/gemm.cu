@@ -9,7 +9,8 @@
 //   warp 8      TMA producer   cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx; it runs ahead into
 //               the next tile while the consumers are in their epilogue.  16-bit row output: after a tile's last k block
 //               it loads the tile's residual into the staging tile, and once the consumers have filled the staging tile
-//               it writes it out with TMA stores (rows past M / H / B are clipped by the tensor map bounds).
+//               it writes it out with TMA stores (rows past M / H / B are clipped by the tensor map bounds).  Head-split
+//               output (Q/K rows, V^T) is written the same way, one tensor map per segment (tmO, tmR, tmS).
 // LoRA fusion (edlora.py:244-246): the rank-padded down matrix [16, K] rides along as 16 extra W rows of the stage, and a
 // second wgmma (m64n16k16) on the same A descriptor produces t = x * down^T; the epilogue adds t * (alpha*up)^T.
 // Convolution: the A tile is a TW x TH x TB pixel patch of the NHWC activation fetched by a 4-D tensor map at
@@ -68,6 +69,8 @@ struct GemmDev {
   int epi_tma;         // 16-bit row output TMA can address: staged epilogue written by TMA stores (tensor map tmO)
   int res_tma;         // epi_tma and the residual is prefetched into the staging tile by TMA (tensor map tmR)
   int epi_lgw;         // log2 of the staging box width in columns (5: row output, 4: GEGLU)
+  int epi_heads;       // epi_tma for head-split output: copy-out staging layout, one tensor map per segment (tmO, tmR, tmS)
+  int nseg;            // head-split segments (N / (heads * head_dim))
   int epi_copy;        // other 16-bit output (head-split, unaligned rows): staged epilogue, copied out by the consumers
   unsigned long long* tl;   // optional timeline buffer (mos_debug_set_timeline)
   int* counters;       // split-K with in-kernel finalize: one arrival counter per output tile (zero between launches)
@@ -135,16 +138,30 @@ __device__ __forceinline__ uint32_t epi_off(int r, int c, int lgw) {
 }
 
 // Copy-out staging layout (head-split output, and row output whose destination TMA cannot address): 20 regions of 2 KB,
-// one per 8-column group.  Row-major groups hold row r's 8 columns at r * 16; transposed groups (V^T columns) hold
-// column c's 128 rows as 16 chunks of 8 rows, chunk index XOR-ed with c % 8, so that both the fragment writes and the
-// 16-byte chunk reads of a warp touch distinct banks.
+// one per 8-column group.  Row-major groups hold row r's 8 columns at r * 16: the smem image of an (8 columns, 128 rows)
+// TMA box.  Transposed groups (V^T columns) hold two 1 KB halves of 64 rows; in a half, column c's 64 rows are a 128-byte
+// line of 8 chunks of 8 rows at c % 8 * 128, chunk index XOR-ed with c % 8: the SWIZZLE_128B smem image of a (64 rows,
+// 8 columns) TMA box.  Both the fragment writes and the 16-byte chunk reads of a warp touch distinct banks.
 __device__ __forceinline__ uint32_t cp_off(int r, int c, bool tr) {
   const int k = c >> 3, cc = c & 7;
-  return tr ? (k << 11) + (cc << 8) + ((((r >> 3) ^ cc) & 15) << 4) + ((r & 7) << 1) : (k << 11) + (r << 4) + (cc << 1);
+  return tr ? (k << 11) + ((r >> 6) << 10) + (cc << 7) + ((((r >> 3) ^ cc) & 7) << 4) + ((r & 7) << 1)
+            : (k << 11) + (r << 4) + (cc << 1);
 }
-// head-split output: global column nc belongs to a V^T segment
-__device__ __forceinline__ bool col_transposed(const GemmDev& p, int nc) {
-  return p.out_mode == MOS_OUT_HEADS && p.seg_kind[nc / (p.heads * p.head_dim)] == MOS_SEG_TRANSPOSED;
+// head-split output: bit k is set when 8-column group k of the tile at column n0 belongs to a V^T segment
+__device__ __forceinline__ uint32_t transposed_groups(const GemmDev& p, int n0) {
+  if (p.out_mode != MOS_OUT_HEADS) return 0u;
+  const int seg_len = p.heads * p.head_dim;
+  int seg = n0 / seg_len, c = n0 - seg * seg_len;
+  uint32_t mask = 0;
+#pragma unroll 1
+  for (int k = 0; k < BN / 8; ++k) {
+    if (p.seg_kind[seg] == MOS_SEG_TRANSPOSED) mask |= 1u << k;
+    if ((c += 8) == seg_len) {
+      c = 0;
+      ++seg;
+    }
+  }
+  return mask;
 }
 // destination of the 16-bit output element (row m, tile column c) of the tile at t
 __device__ __forceinline__ uint16_t* out_elem(const GemmDev& p, const TileCoord& t, long long m, int c) {
@@ -193,7 +210,7 @@ template <bool F16, bool LORA>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmL, const __grid_constant__ CUtensorMap tmO,
-            const __grid_constant__ CUtensorMap tmR, const GemmDev p) {
+            const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmS, const GemmDev p) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by SWIZZLE_128B (an offset from smem_raw, so that the compiler keeps the pointer in
   // the shared address space: the epilogue's staging stores then cannot alias global memory)
@@ -220,7 +237,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (LORA) tma_prefetch_desc(&tmL);
     if (p.epi_tma) {
       tma_prefetch_desc(&tmO);
-      if (p.res_tma) tma_prefetch_desc(&tmR);
+      if (p.res_tma || (p.epi_heads && p.nseg > 1)) tma_prefetch_desc(&tmR);
+      if (p.epi_heads && p.nseg > 2) tma_prefetch_desc(&tmS);
     }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);                          // one arrive.expect_tx by the producer
@@ -258,15 +276,49 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if (p.conv) op(epi + (j << (p.epi_lgw + 8)), c0 + j * box_w, t.cw0, t.ch0, t.cb0);
         else op(epi + (j << (p.epi_lgw + 8)), c0 + j * box_w, t.m0, 0, 0);
       };
+      // head-split output of the tile at t: one store per 8-column group (which lies inside one head) from the copy-out
+      // staging layout.  Q/K: an (8 columns, 128 tokens) box, or (8, 64 tokens, 1 head, 2 batches) at 64 tokens per
+      // batch; V^T: two (64 tokens, 8 columns) boxes.  The maps' extents are head_dim and tokens_per_batch, so that the
+      // pad columns, pad rows and pad tokens of the destination are never written.
+      auto heads_store = [&](const TileCoord& t) {
+        const int T = (int)p.tokens_per_batch;
+        const int seg_len = p.heads * p.head_dim;
+        int seg = t.n0 / seg_len;
+        int head = (t.n0 - seg * seg_len) / p.head_dim;
+        int j = t.n0 - seg * seg_len - head * p.head_dim;
+        const int b0 = t.m0 / T, tok0 = t.m0 - b0 * T;
+        const int b1 = (t.m0 + 64) / T, tok1 = t.m0 + 64 - b1 * T;
+        for (int k = 0; k < BN / 8; ++k) {
+          const CUtensorMap* tm = seg == 0 ? &tmO : seg == 1 ? &tmR : &tmS;
+          const uint8_t* s = epi + (k << 11);
+          if (p.seg_kind[seg] == MOS_SEG_ROWS) {
+            tma_store_4d(tm, s, j, tok0, head, b0);
+          } else {
+            tma_store_4d(tm, s, tok0, j, head, b0);
+            tma_store_4d(tm, s + 1024, tok1, j, head, b1);
+          }
+          if ((j += 8) == p.head_dim) {
+            j = 0;
+            if (++head == p.heads) {
+              head = 0;
+              ++seg;
+            }
+          }
+        }
+      };
       // write out item i (tile t) once the consumers have staged it; returns when the staging tile may be reused
       auto epi_store = [&](const TileCoord& t, int i) {
         mbar_wait_hint(&epi_full, i & 1);
-        const int c0 = p.geglu ? t.n0 / 2 : t.n0;
-        for (int j = 0; j < EPI_BOXES; ++j)
-          epi_box(t, c0, j, [&](const uint8_t* s, int x, int y, int z, int w) {
-            if (p.conv) tma_store_4d(&tmO, s, x, y, z, w);
-            else tma_store_2d(&tmO, s, x, y);
-          });
+        if (p.epi_heads) {
+          heads_store(t);
+        } else {
+          const int c0 = p.geglu ? t.n0 / 2 : t.n0;
+          for (int j = 0; j < EPI_BOXES; ++j)
+            epi_box(t, c0, j, [&](const uint8_t* s, int x, int y, int z, int w) {
+              if (p.conv) tma_store_4d(&tmO, s, x, y, z, w);
+              else tma_store_2d(&tmO, s, x, y);
+            });
+        }
         bulk_commit();
         bulk_wait_read_all();
         if (i == 0) stamp(5);
@@ -399,6 +451,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       // ---- epilogue from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e).  16-bit
       // output (rows, GEGLU, head-split) goes to the staging tile; only fp32 output and split-K partials go to global.
+      const uint32_t trmask = transposed_groups(p, t.n0);
+      const bool row_boxes = p.epi_tma && !p.epi_heads;    // staging layout: epi_off (else cp_off)
+      // LoRA segment of the tile's first column, and that column's offset inside it (segments are multiples of 16
+      // columns wide, so every 8-column group lies inside one)
+      const int lseg = (int)p.lora_seg;
+      const int lseg0 = LORA ? t.n0 / lseg : 0;
+      const int lcol0 = t.n0 - lseg0 * lseg;
       if (p.epi_tma) mbar_wait(&epi_ready, it & 1);
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
@@ -430,11 +489,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               }
               o[e] = a * gelu_erf(g);
             }
-            *reinterpret_cast<uint32_t*>(epi + (p.epi_tma ? epi_off(r, na, p.epi_lgw) : cp_off(r, na, false))) =
+            *reinterpret_cast<uint32_t*>(epi + (row_boxes ? epi_off(r, na, p.epi_lgw) : cp_off(r, na, false))) =
                 pack16x2<F16>(o[0], o[1]);
           }
         } else {
-          int seg = -1;                             // LoRA segment whose rank values are in tt
+          int seg = lseg0, scol = lcol0;            // LoRA segment of group i, and the group's column inside it
           float4 tt = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
           for (int i = 0; i < BN / 8; ++i) {
@@ -443,13 +502,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
             for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + s_bias[bs][8 * i + cq + e];
             if constexpr (LORA) {
-              // segments are multiples of 16 columns wide: seg is the same for the whole 8-column group, so uniform
-              // over the warp, and it changes at most 3 times along the tile
-              const int sg = nc / (int)p.lora_seg;
-              if (sg != seg) {
-                seg = sg;
-                tt = lora_ranks(lacc, hr, sg, lane);
+              // seg is uniform over the warp, and it changes at most 3 times along the tile
+              if (scol == lseg) {
+                scol = 0;
+                ++seg;
               }
+              if (i == 0 || scol == 0) tt = lora_ranks(lacc, hr, seg, lane);
+              scol += 8;
 #pragma unroll
               for (int e = 0; e < 2; ++e) o[e] += lora_term(tt, s_lup[8 * i + cq + e]);
             }
@@ -463,9 +522,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 o[1] += f.y;
               }
               const uint32_t v = pack16x2<F16>(o[0], o[1]);
-              if (p.epi_tma) {
+              if (row_boxes) {
                 *reinterpret_cast<uint32_t*>(epi + epi_off(r, cl, p.epi_lgw)) = v;
-              } else if (!col_transposed(p, nc)) {
+              } else if (!((trmask >> i) & 1u)) {
                 *reinterpret_cast<uint32_t*>(epi + cp_off(r, cl, false)) = v;
               } else {
                 *reinterpret_cast<uint16_t*>(epi + cp_off(r, cl, true)) = (uint16_t)(v & 0xFFFFu);
@@ -497,7 +556,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           const int groups = (p.geglu ? BN / 2 : BN) / 8;
           for (int idx = et; idx < groups * BM; idx += CONSUMER_THREADS) {
             const int k = idx / BM, rs = idx % BM;
-            const bool tr = col_transposed(p, t.n0 + 8 * k);
+            const bool tr = (trmask >> k) & 1u;
             const int r0 = tr ? (rs & ~7) : rs;           // V^T: 8 rows of column 8k + rs % 8
             const int c0 = tr ? 8 * k + (rs & 7) : 8 * k;
             const uint8_t* src = epi + cp_off(r0, c0, tr);
@@ -715,10 +774,11 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
 
   GemmDev p;
   memset(&p, 0, sizeof(p));
-  CUtensorMap tmA, tmB, tmL, tmO, tmR;
+  CUtensorMap tmA, tmB, tmL, tmO, tmR, tmS;
   memset(&tmL, 0, sizeof(tmL));
   memset(&tmO, 0, sizeof(tmO));
   memset(&tmR, 0, sizeof(tmR));
+  memset(&tmS, 0, sizeof(tmS));
   p.M = (int)a->M;
   p.N = (int)a->N;
   p.conv = a->conv;
@@ -826,16 +886,59 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   // Every 16-bit output goes through the staging tile.  Row output (with GEGLU and residual) that TMA can address (16-byte
   // aligned base, row pitch a multiple of 8 elements) is written by TMA stores, its residual prefetched by TMA when that
   // is addressable too: tensor maps with the tile's row geometry (plain [M, cols], conv [B, H, W, cols]), one box per
-  // staging box.  Head-split output and other row output are copied out of the staging tile by the consumers.
+  // staging box.  Head-split output is written by TMA stores as well when every 64-row half of a tile lies inside one
+  // batch and a 128-row tile inside one batch or two whole ones (tokens_per_batch 64 or a multiple of 128), and every
+  // segment is addressable: one tensor map per segment, Q/K [batch, head, token, j] and V^T [batch, head, j, token] with
+  // the extents head_dim and tokens_per_batch.  Other head-split output (the 77-token text K/V) and other row output are
+  // copied out of the staging tile by the consumers.  MOS_GEMM_HEADS_COPY=1 sends all head-split output that way.
+  static int heads_copy_env = -1;
+  if (heads_copy_env < 0) {
+    const char* hc = getenv("MOS_GEMM_HEADS_COPY");
+    heads_copy_env = (hc && atoi(hc) != 0) ? 1 : 0;
+  }
   const uint64_t cols = (uint64_t)(a->geglu ? a->N / 2 : a->N);
   auto tma_rows = [&](const void* base, long long ld) {
     return base != nullptr && ld >= (long long)cols && ld % 8 == 0 && is_aligned(base, 16);
   };
+  const long long T = p.tokens_per_batch;
+  const int nseg = a->out_mode == MOS_OUT_HEADS ? (int)(a->N / ((long long)a->heads * a->head_dim)) : 0;
+  bool heads_tma = a->out_mode == MOS_OUT_HEADS && !heads_copy_env && (T == 64 || T % 128 == 0) && a->M % T == 0;
+  for (int s = 0; s < nseg && heads_tma; ++s) {
+    const bool tr = a->seg_kind[s] == MOS_SEG_TRANSPOSED;
+    heads_tma = a->seg_ptr[s] != nullptr && is_aligned(a->seg_ptr[s], 16) && a->seg_rows_pad[s] >= T &&
+                (tr ? a->dv_pad >= a->head_dim && a->seg_rows_pad[s] % 8 == 0
+                    : a->dpad >= a->head_dim && a->dpad % 8 == 0);
+  }
   if (a->geglu || a->out_mode == MOS_OUT_HEADS) p.residual = nullptr;   // neither takes a residual
-  p.epi_tma = (a->out_mode == MOS_OUT_BF16 && splits == 1 && tma_rows(a->out, a->ldc)) ? 1 : 0;
+  p.epi_heads = heads_tma ? 1 : 0;
+  p.nseg = nseg;
+  p.epi_tma = ((a->out_mode == MOS_OUT_BF16 && splits == 1 && tma_rows(a->out, a->ldc)) || heads_tma) ? 1 : 0;
   p.res_tma = (p.epi_tma && p.residual != nullptr && tma_rows(a->residual, a->ldr)) ? 1 : 0;
   p.epi_copy = (a->out_mode != MOS_OUT_F32 && splits == 1 && !p.epi_tma) ? 1 : 0;
-  if (p.epi_tma) {
+  if (heads_tma) {
+    CUtensorMap* maps[3] = {&tmO, &tmR, &tmS};
+    const uint64_t B = (uint64_t)(a->M / T), H = (uint64_t)a->heads, d = (uint64_t)a->head_dim;
+    for (int s = 0; s < nseg; ++s) {
+      const uint64_t rows = (uint64_t)a->seg_rows_pad[s];
+      int rc;
+      if (a->seg_kind[s] == MOS_SEG_TRANSPOSED) {
+        const uint64_t pitch = rows * 2;
+        uint64_t dims[4] = {(uint64_t)T, d, H, B};
+        uint64_t str[3] = {pitch, (uint64_t)a->dv_pad * pitch, H * a->dv_pad * pitch};
+        uint32_t box[4] = {64, 8, 1, 1};
+        rc = encode_tmap(maps[s], a->seg_ptr[s], 2, 4, dims, str, box, 3);
+      } else {
+        const uint64_t pitch = (uint64_t)a->dpad * 2;
+        const uint32_t bt = T == 64 ? 64 : 128;
+        uint64_t dims[4] = {d, (uint64_t)T, H, B};
+        uint64_t str[3] = {pitch, rows * pitch, H * rows * pitch};
+        uint32_t box[4] = {8, bt, 1, BM / bt};
+        rc = encode_tmap(maps[s], a->seg_ptr[s], 2, 4, dims, str, box, 0);
+      }
+      if (rc) return rc;
+    }
+  }
+  if (p.epi_tma && !p.epi_heads) {
     p.epi_lgw = a->geglu ? 4 : 5;
     const uint32_t bw = 1u << p.epi_lgw;
     const int swz = a->geglu ? 1 : 2;        // SWIZZLE_32B / SWIZZLE_64B: rows of 2 bw bytes (epi_off)
@@ -910,7 +1013,7 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   const int units = p.total_items < num_sms ? p.total_items : num_sms;
   auto kern = f16 ? (lora ? gemm_kernel<true, true> : gemm_kernel<true, false>)
                   : (lora ? gemm_kernel<false, true> : gemm_kernel<false, false>);
-  MOS_CHECK_CUDA(launch_pdl(kern, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA, tmB, tmL, tmO, tmR, p));
+  MOS_CHECK_CUDA(launch_pdl(kern, dim3((unsigned)units), dim3(NUM_THREADS), (size_t)smem_bytes, stream, tmA, tmB, tmL, tmO, tmR, tmS, p));
   return MOS_OK;
 }
 
