@@ -89,9 +89,12 @@ typedef struct mos_gemm_args {
 
 int mos_gemm_bf16(const mos_gemm_args* args, void* stream);
 
-/* Profiling aid: register a device buffer of 64 uint64 (or NULL to disable); the first 8 CTAs of every subsequent
- * mos_gemm_bf16 launch store %globaltimer stamps [start, setup done, pdl wait done, first TMA landed, epilogue
- * prefetch done, accumulators ready, accumulators drained, tile written]. */
+/* Profiling aid: register a device buffer of 8 x 16 uint64 (or NULL to disable); the first 8 CTAs of every subsequent
+ * mos_gemm_bf16 launch store %globaltimer stamps (ns) into their 16 slots: [0] start, [1] barriers initialised,
+ * [2] producer start, [3] first k block landed; first tile: [4] accumulators ready, [6] epilogue operands in shared
+ * memory, [7] staging tile free, [8] staging tile written, [9] producer saw it written, [10] stores issued, [5] tile
+ * written; second tile: [11] accumulators ready, [12] operands in shared memory, [13] staging tile free, [14] staging
+ * tile written, [15] tile written.  Slots a launch does not reach are left as they were. */
 int mos_debug_set_timeline(void* buf);
 
 /* Sum split-K partials and apply bias / bias_batch / residual -> bf16 [M, ldc]. */

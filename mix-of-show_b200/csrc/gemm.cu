@@ -38,6 +38,8 @@ constexpr int EPI_BATCHES = 5;   // batches one 128-row tile can span (plain: ro
 // 16 (GEGLU's 80 output columns, SWIZZLE_32B), each box the smem image of one TMA store / residual load.
 constexpr int EPI_BYTES = BM * BN * 2;                   // 40960
 constexpr int EPI_BOXES = 5;
+constexpr int EPI_LGW_ROWS = 5;                          // log2 of the box width: row output
+constexpr int EPI_LGW_GEGLU = 4;                         // GEGLU (80 output columns per tile)
 
 struct GemmDev {
   int M, N;
@@ -68,10 +70,11 @@ struct GemmDev {
   int accum;           // MOS_OUT_F32: out += result (Gram accumulation)
   int epi_tma;         // 16-bit row output TMA can address: staged epilogue written by TMA stores (tensor map tmO)
   int res_tma;         // epi_tma and the residual is prefetched into the staging tile by TMA (tensor map tmR)
-  int epi_lgw;         // log2 of the staging box width in columns (5: row output, 4: GEGLU)
+  int epi_lgw;         // log2 of the staging box width in columns (EPI_LGW_ROWS, EPI_LGW_GEGLU)
   int epi_heads;       // epi_tma for head-split output: copy-out staging layout, one tensor map per segment (tmO, tmR, tmS)
   int nseg;            // head-split segments (N / (heads * head_dim))
   int epi_copy;        // other 16-bit output (head-split, unaligned rows): staged epilogue, copied out by the consumers
+  int epi_mode;        // EpiMode of the launch's tiles
   unsigned long long* tl;   // optional timeline buffer (mos_debug_set_timeline)
   int* counters;       // split-K with in-kernel finalize: one arrival counter per output tile (zero between launches)
   const uint8_t* pf;   // optional: bytes to pull into L2 for a LATER launch (the next layer's weights), see mos_gemm_args
@@ -83,14 +86,20 @@ __device__ __forceinline__ void epi_bar() {  // consumer warps only
 }
 
 // ---- optional in-kernel timeline (profiling aid): when a buffer is registered through mos_debug_set_timeline, the
-// first 8 CTAs of every gemm launch record %globaltimer stamps (ns) at their phase boundaries.  The pointer travels in
+// first 8 CTAs of every gemm launch record %globaltimer stamps (ns) at their phase boundaries, TL_SLOTS per CTA:
+//   0 CTA start, 1 barriers initialised, 2 producer start, 3 first k block landed (consumer)
+//   first tile:  4 accumulators ready, 6 epilogue operands in shared memory, 7 epi_ready passed, 8 staging tile
+//                written (epi_full arrived), 9 epi_full observed by the producer, 10 stores issued, 5 tile written
+//   second tile: 11 accumulators ready, 12 operands in shared memory, 13 epi_ready passed, 14 staging tile written,
+//                15 tile written  The pointer travels in
 // the kernel parameters (constant bank): a __device__ global would cost an L2 round trip at every stamp site.
+constexpr int TL_SLOTS = 16;
 #define stamp(slot)                                                       \
   do {                                                                    \
     if (p.tl != nullptr && blockIdx.x < 8) {                              \
       unsigned long long t_;                                              \
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));              \
-      p.tl[blockIdx.x * 8 + (slot)] = t_;                                 \
+      p.tl[blockIdx.x * TL_SLOTS + (slot)] = t_;                          \
     }                                                                     \
   } while (0)
 
@@ -126,15 +135,6 @@ __device__ __forceinline__ bool row_coord(const GemmDev& p, const TileCoord& t, 
   m = (long long)t.m0 + r;
   b = (int)(m / p.rows_per_batch);
   return m < p.M;
-}
-
-// Byte offset of (tile row r, output column c) in the staging tile: box c / w, rows of 2w bytes, the 16-byte chunk index
-// XOR-ed with address bits [7, 7 + log2(w/8)) of the row, which is the TMA SWIZZLE_32B / SWIZZLE_64B pattern.  A warp's
-// store of one fragment column pair (8 rows x 16 bytes) then touches 32 distinct banks.
-__device__ __forceinline__ uint32_t epi_off(int r, int c, int lgw) {
-  const int cin = c & ((1 << lgw) - 1);
-  const int chunk = (cin >> 3) ^ ((r >> (6 - lgw)) & ((1 << (lgw - 3)) - 1));
-  return ((c >> lgw) << (lgw + 8)) + (r << (lgw + 1)) + (chunk << 4) + ((cin & 7) << 1);
 }
 
 // Copy-out staging layout (head-split output, and row output whose destination TMA cannot address): 20 regions of 2 KB,
@@ -202,6 +202,169 @@ __device__ __forceinline__ float4 lora_ranks(const float (&lacc)[LORA_N / 2], in
 }
 // LoRA term of an output column: t[4 ranks of the column's segment] . (alpha * up)[column]
 __device__ __forceinline__ float lora_term(float4 t, float4 u) { return t.x * u.x + t.y * u.y + t.z * u.z + t.w * u.w; }
+
+// Output path of a tile's epilogue, fixed per launch by the host (GemmDev::epi_mode), except EPI_HEADS_T, which a
+// head-split tile takes when one of its 8-column groups belongs to a V^T segment.
+enum EpiMode {
+  EPI_ROWS,              // 16-bit rows (also head-split Q/K rows) into the staging tile
+  EPI_ROWS_RES_SMEM,     // + residual, prefetched into the staging tile by TMA
+  EPI_ROWS_RES_GLOBAL,   // + residual, read from global memory (TMA cannot address it)
+  EPI_HEADS_T,           // head-split, copy-out layout, V^T groups transposed
+  EPI_GEGLU,             // a * gelu(gate) rows (80 of the tile's 160 columns)
+  EPI_F32,               // fp32 rows to global (optionally accumulated)
+  EPI_PARTIAL,           // split-K fp32 partial tile to the workspace
+};
+
+struct EpiArgs {
+  uint8_t* epi;          // staging tile
+  const float* s_bias;   // [EPI_BATCHES][BN]
+  const float4* s_lup;   // [BN] (LoRA)
+  int rA, cq, lane, b_lo;
+};
+
+// Staging layouts of 16-bit row output (byte offset of tile row r, column c = 8i + cq; the fragment of group i holds
+// columns 8i + cq, 8i + cq + 1):
+//  - column boxes (TMA-store row output): box c / w of [128 rows][w columns], w = 1 << EPI_LGW_ROWS (32) or
+//    1 << EPI_LGW_GEGLU (16), rows of 2w bytes, the 16-byte chunk index XOR-ed with address bits [7, 7 + log2(w/8)) of
+//    the row: the TMA SWIZZLE_64B / SWIZZLE_32B pattern.  A warp's store of one fragment column pair (8 rows x 16 bytes)
+//    then touches 32 distinct banks.
+//  - copy-out groups (cp_off): 2 KB per 8-column group.
+// Either way the offset of group i is base[i % G] + (i / G) * (G * 2 KB), G = w / 8 groups per box, with the G bases
+// worked out once per row.
+template <int LGW>
+__device__ __forceinline__ void staging_bases(uint32_t (&base)[(1 << LGW) / 8], bool box, int r, int cq) {
+  constexpr int G = (1 << LGW) / 8;
+  static_assert(G * 2048 == BM * (1 << LGW) * 2, "a box of G groups is G copy-out groups");
+  const uint32_t bx = (r << (LGW + 1)) | (((r >> (6 - LGW)) & (G - 1)) << 4) | (cq << 1);
+#pragma unroll
+  for (int k = 0; k < G; ++k) base[k] = box ? bx ^ (k << 4) : cp_off(r, 8 * k + cq, false);
+}
+
+// Epilogue of one tile from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e).  Every
+// index into acc / lacc is a compile-time constant.  The bias and LoRA terms of a column group are added by one piece of
+// code shared by every path that takes them; the group's store is its path's own compile-time instantiation
+// (epi_store<MODE>, no runtime tests inside), picked by warp-uniform branches.  These also keep each group's
+// shared-memory operand reads next to the group's store: hoisted above all 20 stores, they would hold 40 registers.
+struct EpiRow {
+  uint32_t base[(1 << EPI_LGW_ROWS) / 8];   // staging_bases of the row
+  uint32_t tbase0, tbase1;                 // V^T groups (EPI_HEADS_T): column cq + e, 2-byte stores (cp_off transposed)
+  const __nv_bfloat16* res;                // EPI_ROWS_RES_GLOBAL: residual of column n0 + cq
+  float* fout;                             // EPI_F32: output of column n0 + cq
+};
+template <int MODE, bool F16>
+__device__ __forceinline__ void epi_store(const GemmDev& p, const EpiArgs& ea, const EpiRow& er, int i, float o0, float o1,
+                                          uint32_t trmask) {
+  constexpr int G = (1 << EPI_LGW_ROWS) / 8;
+  uint8_t* dst = ea.epi + er.base[i % G] + (i / G) * (G << 11);
+  if constexpr (MODE == EPI_F32) {
+    float2* d2 = reinterpret_cast<float2*>(er.fout + 8 * i);
+    float2 r2 = make_float2(o0, o1);
+    if (p.accum) {
+      const float2 old = *d2;
+      r2.x += old.x;
+      r2.y += old.y;
+    }
+    *d2 = r2;
+    return;
+  }
+  if constexpr (MODE == EPI_ROWS_RES_SMEM || MODE == EPI_ROWS_RES_GLOBAL) {
+    const float2 f = unpack16x2<F16>(MODE == EPI_ROWS_RES_SMEM ? *reinterpret_cast<const uint32_t*>(dst)
+                                                               : *reinterpret_cast<const uint32_t*>(er.res + 8 * i));
+    o0 += f.x;
+    o1 += f.y;
+  }
+  const uint32_t v = pack16x2<F16>(o0, o1);
+  if (MODE == EPI_HEADS_T && ((trmask >> i) & 1u)) {
+    *reinterpret_cast<uint16_t*>(ea.epi + er.tbase0 + (i << 11)) = (uint16_t)(v & 0xFFFFu);
+    *reinterpret_cast<uint16_t*>(ea.epi + er.tbase1 + (i << 11)) = (uint16_t)(v >> 16);
+  } else {
+    *reinterpret_cast<uint32_t*>(dst) = v;
+  }
+}
+
+template <bool F16, bool LORA>
+__device__ __forceinline__ void epilogue(const GemmDev& p, const TileCoord& t, const EpiArgs& ea,
+                                         const float (&acc)[BN / 2],
+                                         const float (&lacc)[LORA_N / 2], uint32_t trmask, int mode) {
+  // LoRA segment of the tile's first column, and that column's offset inside it.  Segments and tiles start at
+  // multiples of 16 columns, so a segment can only change at an even group.
+  const int lseg = (int)p.lora_seg;
+  const int lseg0 = LORA ? t.n0 / lseg : 0;
+  const int lcol0 = t.n0 - lseg0 * lseg;
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int r = ea.rA + 8 * hr;
+    long long m;
+    int b;
+    if (!row_coord(p, t, r, m, b)) continue;
+    const float* sb = ea.s_bias + (p.bias_batch ? b - ea.b_lo : 0) * BN + ea.cq;   // s_bias slot of the row
+    const float4* su = ea.s_lup + ea.cq;
+    if (mode == EPI_PARTIAL) {                      // (the host rejects LoRA together with split-K)
+      if constexpr (!LORA) {
+        float* dst = p.partial + ((long long)t.split * p.M + m) * p.N + t.n0 + ea.cq;
+#pragma unroll
+        for (int i = 0; i < BN / 8; ++i)
+          *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
+      }
+      continue;
+    }
+    if (mode == EPI_GEGLU) {
+      // tile columns [0,80) = a, [80,160) = gate for the same 80 outputs (columns n0/2 + [0,80) of the output)
+      constexpr int G = (1 << EPI_LGW_GEGLU) / 8;
+      uint32_t base[G];
+      staging_bases<EPI_LGW_GEGLU>(base, p.epi_tma && !p.epi_heads, r, ea.cq);
+      float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if constexpr (LORA) t0 = lora_ranks(lacc, hr, 0, ea.lane);
+#pragma unroll
+      for (int i = 0; i < BN / 16; ++i) {
+        float o[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float a = acc[4 * i + 2 * hr + e] + sb[8 * i + e];
+          float g = acc[4 * (i + BN / 16) + 2 * hr + e] + sb[8 * i + BN / 2 + e];
+          if constexpr (LORA) {
+            a += lora_term(t0, su[8 * i + e]);
+            g += lora_term(t0, su[8 * i + BN / 2 + e]);
+          }
+          o[e] = a * gelu_erf(g);
+        }
+        *reinterpret_cast<uint32_t*>(ea.epi + base[i % G] + (i / G) * (G << 11)) = pack16x2<F16>(o[0], o[1]);
+      }
+      continue;
+    }
+    // every other path: acc + bias (+ LoRA term), then the path's store
+    EpiRow er;
+    staging_bases<EPI_LGW_ROWS>(er.base, p.epi_tma && !p.epi_heads, r, ea.cq);
+    er.tbase0 = cp_off(r, ea.cq, true);
+    er.tbase1 = cp_off(r, ea.cq + 1, true);
+    er.res = p.residual + m * p.ldr + t.n0 + ea.cq;
+    er.fout = reinterpret_cast<float*>(p.out) + m * p.ldc + t.n0 + ea.cq;
+    int seg = lseg0, scol = lcol0;                  // LoRA segment of group i, and the group pair's column inside it
+    float4 tt = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (LORA) tt = lora_ranks(lacc, hr, seg, ea.lane);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      float o[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + sb[8 * i + e];
+      if constexpr (LORA) {
+        if (i > 0 && i % 2 == 0 && (scol += 16) == lseg) {   // seg is uniform over the warp
+          scol = 0;
+          tt = lora_ranks(lacc, hr, ++seg, ea.lane);
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) o[e] += lora_term(tt, su[8 * i + e]);
+      }
+      // (direct branches on the uniform mode, in the order of how often the denoise step takes the paths: a jump
+      // table's indirect branch per group costs more than the compares)
+      if (mode == EPI_ROWS) epi_store<EPI_ROWS, F16>(p, ea, er, i, o[0], o[1], trmask);
+      else if (mode == EPI_ROWS_RES_SMEM) epi_store<EPI_ROWS_RES_SMEM, F16>(p, ea, er, i, o[0], o[1], trmask);
+      else if (mode == EPI_HEADS_T) epi_store<EPI_HEADS_T, F16>(p, ea, er, i, o[0], o[1], trmask);
+      else if (mode == EPI_ROWS_RES_GLOBAL) epi_store<EPI_ROWS_RES_GLOBAL, F16>(p, ea, er, i, o[0], o[1], trmask);
+      else epi_store<EPI_F32, F16>(p, ea, er, i, o[0], o[1], trmask);
+    }
+  }
+}
 
 // F16: 16-bit type of A, of the row / head-split outputs and of the residual (fp16 or bf16).
 // LORA: the fused LoRA branch is present (a template parameter, so that the k16 wgmma chain of a k block is straight-line
@@ -309,6 +472,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       // write out item i (tile t) once the consumers have staged it; returns when the staging tile may be reused
       auto epi_store = [&](const TileCoord& t, int i) {
         mbar_wait_hint(&epi_full, i & 1);
+        if (i == 0) stamp(9);
         if (p.epi_heads) {
           heads_store(t);
         } else {
@@ -320,8 +484,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             });
         }
         bulk_commit();
+        if (i == 0) stamp(10);
         bulk_wait_read_all();
         if (i == 0) stamp(5);
+        if (i == 1) stamp(15);
       };
       int stage = 0;
       uint32_t phase = 0;
@@ -433,7 +599,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      if (et == 0 && it == 0) stamp(4);
+      if (et == 0 && it < 2) stamp(it == 0 ? 4 : 11);
       int b_lo;                                            // batch of the tile's first row (s_bias slot 0)
       {
         long long m0;
@@ -449,100 +615,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (et < BN) s_lup[et] = __ldg(reinterpret_cast<const float4*>(p.lora_up) + t.n0 + et);
         epi_bar();
       }
-      // ---- epilogue from the accumulator fragment: d[4i + 2hr + e] = (row rA + 8 hr, column 8i + cq + e).  16-bit
-      // output (rows, GEGLU, head-split) goes to the staging tile; only fp32 output and split-K partials go to global.
+      if (et == 0 && it < 2) stamp(it == 0 ? 6 : 12);
+      // ---- epilogue from the accumulator fragment.  16-bit output (rows, GEGLU, head-split) goes to the staging tile;
+      // only fp32 output and split-K partials go to global.  Each output path is its own straight-line code (the
+      // launch's path is a kernel parameter; head-split tiles with V^T columns take their own), so that a tile runs
+      // only the instructions of its path.
       const uint32_t trmask = transposed_groups(p, t.n0);
-      const bool row_boxes = p.epi_tma && !p.epi_heads;    // staging layout: epi_off (else cp_off)
-      // LoRA segment of the tile's first column, and that column's offset inside it (segments are multiples of 16
-      // columns wide, so every 8-column group lies inside one)
-      const int lseg = (int)p.lora_seg;
-      const int lseg0 = LORA ? t.n0 / lseg : 0;
-      const int lcol0 = t.n0 - lseg0 * lseg;
       if (p.epi_tma) mbar_wait(&epi_ready, it & 1);
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int r = rA + 8 * hr;
-        long long m;
-        int b;
-        if (!row_coord(p, t, r, m, b)) continue;
-        const int bs = p.bias_batch ? b - b_lo : 0;     // s_bias slot of the row
-        if (!LORA && p.splits > 1) {               // (the host rejects LoRA together with split-K)
-          float* dst = p.partial + ((long long)t.split * p.M + m) * p.N + t.n0 + cq;
-#pragma unroll
-          for (int i = 0; i < BN / 8; ++i)
-            *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
-        } else if (p.geglu) {
-          // tile columns [0,80) = a, [80,160) = gate for the same 80 outputs (columns n0/2 + [0,80) of the output)
-          float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if constexpr (LORA) t0 = lora_ranks(lacc, hr, 0, lane);
-#pragma unroll
-          for (int i = 0; i < BN / 16; ++i) {
-            const int na = 8 * i + cq, ng = na + BN / 2;
-            float o[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              float a = acc[4 * i + 2 * hr + e] + s_bias[bs][na + e];
-              float g = acc[4 * (i + BN / 16) + 2 * hr + e] + s_bias[bs][ng + e];
-              if constexpr (LORA) {
-                a += lora_term(t0, s_lup[na + e]);
-                g += lora_term(t0, s_lup[ng + e]);
-              }
-              o[e] = a * gelu_erf(g);
-            }
-            *reinterpret_cast<uint32_t*>(epi + (row_boxes ? epi_off(r, na, p.epi_lgw) : cp_off(r, na, false))) =
-                pack16x2<F16>(o[0], o[1]);
-          }
-        } else {
-          int seg = lseg0, scol = lcol0;            // LoRA segment of group i, and the group's column inside it
-          float4 tt = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int i = 0; i < BN / 8; ++i) {
-            const int nc = t.n0 + 8 * i + cq;       // global column of the pair (nc, nc + 1)
-            float o[2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e) o[e] = acc[4 * i + 2 * hr + e] + s_bias[bs][8 * i + cq + e];
-            if constexpr (LORA) {
-              // seg is uniform over the warp, and it changes at most 3 times along the tile
-              if (scol == lseg) {
-                scol = 0;
-                ++seg;
-              }
-              if (i == 0 || scol == 0) tt = lora_ranks(lacc, hr, seg, lane);
-              scol += 8;
-#pragma unroll
-              for (int e = 0; e < 2; ++e) o[e] += lora_term(tt, s_lup[8 * i + cq + e]);
-            }
-            const int cl = 8 * i + cq;              // tile column of the pair
-            if (p.out_mode != MOS_OUT_F32) {
-              if (p.residual) {                     // (row output only: the host drops it for head-split output)
-                const float2 f = unpack16x2<F16>(
-                    p.res_tma ? *reinterpret_cast<const uint32_t*>(epi + epi_off(r, cl, p.epi_lgw))
-                              : *reinterpret_cast<const uint32_t*>(p.residual + m * p.ldr + nc));
-                o[0] += f.x;
-                o[1] += f.y;
-              }
-              const uint32_t v = pack16x2<F16>(o[0], o[1]);
-              if (row_boxes) {
-                *reinterpret_cast<uint32_t*>(epi + epi_off(r, cl, p.epi_lgw)) = v;
-              } else if (!((trmask >> i) & 1u)) {
-                *reinterpret_cast<uint32_t*>(epi + cp_off(r, cl, false)) = v;
-              } else {
-                *reinterpret_cast<uint16_t*>(epi + cp_off(r, cl, true)) = (uint16_t)(v & 0xFFFFu);
-                *reinterpret_cast<uint16_t*>(epi + cp_off(r, cl + 1, true)) = (uint16_t)(v >> 16);
-              }
-            } else {
-              float2* dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + m * p.ldc + nc);
-              float2 r2 = make_float2(o[0], o[1]);
-              if (p.accum) {
-                const float2 old = *dst;
-                r2.x += old.x;
-                r2.y += old.y;
-              }
-              *dst = r2;
-            }
-          }
-        }
-      }
+      if (et == 0 && it < 2) stamp(it == 0 ? 7 : 13);
+      const EpiArgs ea{epi, &s_bias[0][0], s_lup, rA, cq, lane, b_lo};
+      epilogue<F16, LORA>(p, t, ea, acc, lacc, trmask, trmask != 0u ? (int)EPI_HEADS_T : p.epi_mode);
+      if (et == 0 && it < 2) stamp(it == 0 ? 8 : 14);
       if (p.epi_tma) {
         fence_proxy_async_smem();                          // this thread's staging writes -> the TMA store's reads
         mbar_arrive(&epi_full);
@@ -581,7 +664,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             }
           }
         }
-        if (et == 0 && it == 0) stamp(5);
+        if (et == 0 && it < 2) stamp(it == 0 ? 5 : 15);
       }
       if (!LORA && p.counters != nullptr) {
         // split-K, in-kernel finalize: publish this item's partial tile (bar.sync ordered every consumer thread's stores
@@ -915,6 +998,12 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
   p.epi_tma = ((a->out_mode == MOS_OUT_BF16 && splits == 1 && tma_rows(a->out, a->ldc)) || heads_tma) ? 1 : 0;
   p.res_tma = (p.epi_tma && p.residual != nullptr && tma_rows(a->residual, a->ldr)) ? 1 : 0;
   p.epi_copy = (a->out_mode != MOS_OUT_F32 && splits == 1 && !p.epi_tma) ? 1 : 0;
+  p.epi_mode = splits > 1                    ? EPI_PARTIAL
+               : a->out_mode == MOS_OUT_F32  ? EPI_F32
+               : a->geglu                    ? EPI_GEGLU
+               : p.residual == nullptr       ? EPI_ROWS
+               : p.res_tma                   ? EPI_ROWS_RES_SMEM
+                                             : EPI_ROWS_RES_GLOBAL;
   if (heads_tma) {
     CUtensorMap* maps[3] = {&tmO, &tmR, &tmS};
     const uint64_t B = (uint64_t)(a->M / T), H = (uint64_t)a->heads, d = (uint64_t)a->head_dim;
@@ -939,9 +1028,9 @@ extern "C" int mos_gemm_bf16(const mos_gemm_args* a, void* stream_) {
     }
   }
   if (p.epi_tma && !p.epi_heads) {
-    p.epi_lgw = a->geglu ? 4 : 5;
+    p.epi_lgw = a->geglu ? EPI_LGW_GEGLU : EPI_LGW_ROWS;
     const uint32_t bw = 1u << p.epi_lgw;
-    const int swz = a->geglu ? 1 : 2;        // SWIZZLE_32B / SWIZZLE_64B: rows of 2 bw bytes (epi_off)
+    const int swz = a->geglu ? 1 : 2;        // SWIZZLE_32B / SWIZZLE_64B: rows of 2 bw bytes (epilogue)
     auto row_map = [&](CUtensorMap* tm, const void* base, long long ld) -> int {
       const uint64_t pitch = (uint64_t)ld * 2;
       if (a->conv) {

@@ -4,10 +4,16 @@ Records every ops.gemm call of one eager step on the real engine buffers, groups
 and replays each group back to back between CUDA events (same arguments, so the same kernel parameters).  Per shape it
 prints us per launch, achieved TFLOP/s (2*M*N*K), and the tensor-rate bound: ceil(items / SMs) * (k blocks per item)
 * 640 cycles (one 128x160x64 k block at 4096 dense 16-bit FLOP/clk/SM) at the card's maximum SM clock.  With the
-in-kernel timeline (mos_debug_set_timeline) it prints the phase split of the first work item of the first 8 CTAs:
-first TMA landed -> accumulators ready -> tile written (stamps 3, 4, 5; medians over the 8 CTAs).  On the TMA-store
-path stamp 5 is taken by the producer warp once the tile has left shared memory; a CTA with several tiles writes a
-tile out only after issuing the next tile's k blocks, so there the last phase includes that wait.
+in-kernel timeline (mos_debug_set_timeline, 16 stamps per CTA, listed in csrc/gemm.cu) it prints the phase split of
+the first work item of the first 8 CTAs (medians over the CTAs that stamped both ends of a phase):
+  tma1   launch -> first k block landed            main   -> accumulators ready
+  ops    -> epilogue operands in shared memory     rdy    -> epi_ready passed (residual landed)
+  stage  -> staging tile written                   wake   -> the producer observed epi_full
+  issue  -> TMA stores issued                      drain  -> the stores have read the staging tile
+  epi    accumulators ready -> tile written (ops + rdy + stage + wake + issue + drain)
+and `epi2`, the same epilogue phase of the second work item in CTAs that run several.  A CTA with several tiles writes
+a tile out only after issuing the next tile's k blocks, so there `epi` includes that wait.  On the copy-out path (no
+TMA stores) the consumers write the tile and `wake`, `issue` and `drain` are empty.
 
 The replay calls ops.gemm, which encodes the tensor maps on the host at every launch: a launch shorter than that host
 work is timed at the host's rate, so compare short launches against the bound with the timeline's phases.
@@ -150,7 +156,8 @@ def main():
         clk_ghz = 1.98
 
     lib = _lib.lib()
-    tl = torch.zeros(8 * 8, dtype=torch.int64, device=dev)
+    TL_SLOTS = 16
+    tl = torch.zeros(8 * TL_SLOTS, dtype=torch.int64, device=dev)
     rows = []
     for calls_g in groups.values():
         A, W, out, kw = calls_g[0]
@@ -174,7 +181,7 @@ def main():
             torch.cuda.synchronize()
         finally:
             _lib.check(lib.mos_debug_set_timeline(None), 'mos_debug_set_timeline')
-        st = tl.view(8, 8).cpu().tolist()
+        st = tl.view(8, TL_SLOTS).cpu().tolist()
         ncta = min(8, items)
 
         def med(a, b):
@@ -184,16 +191,21 @@ def main():
         bound_us = math.ceil(items / n_sm) * kbi * CYCLES_PER_KBLOCK / (clk_ghz * 1e3)
         rows.append(dict(M=M, N=N, K=K, kind=label, count=len(calls_g), items=items, kb_per_item=kbi, us=us,
                          tflops=flops / (us * 1e-6) / 1e12, bound_us=bound_us,
-                         first_tma_us=med(1, 3), mainloop_us=med(3, 4), epilogue_us=med(4, 5)))
+                         first_tma_us=med(1, 3), mainloop_us=med(3, 4), epilogue_us=med(4, 5),
+                         ops_us=med(4, 6), ready_us=med(6, 7), stage_us=med(7, 8), wake_us=med(8, 9),
+                         issue_us=med(9, 10), drain_us=med(10, 5), epilogue2_us=med(11, 15)))
     rows.sort(key=lambda r: -r['us'] * r['count'])
     print(f"card: {info}  SMs {n_sm}  bound clock {clk_ghz:.3f} GHz  launches/step {len(calls)}")
     hdr = (f"{'M':>6} {'N':>5} {'K':>5} {'kind':<18} {'n':>3} {'items':>5} {'kb':>4} {'us':>8} {'TF/s':>6} "
-           f"{'bound':>7} {'tma1':>6} {'main':>7} {'epi':>6}")
+           f"{'bound':>7} {'tma1':>6} {'main':>7} {'epi':>6} {'ops':>6} {'rdy':>6} {'stage':>6} {'wake':>6} "
+           f"{'issue':>6} {'drain':>6} {'epi2':>6}")
     print(hdr)
     for r in rows:
         print(f"{r['M']:>6} {r['N']:>5} {r['K']:>5} {r['kind']:<18} {r['count']:>3} {r['items']:>5} "
               f"{r['kb_per_item']:>4} {r['us']:>8.2f} {r['tflops']:>6.1f} {r['bound_us']:>7.2f} "
-              f"{r['first_tma_us']:>6.2f} {r['mainloop_us']:>7.2f} {r['epilogue_us']:>6.2f}")
+              f"{r['first_tma_us']:>6.2f} {r['mainloop_us']:>7.2f} {r['epilogue_us']:>6.2f} {r['ops_us']:>6.2f} "
+              f"{r['ready_us']:>6.2f} {r['stage_us']:>6.2f} {r['wake_us']:>6.2f} {r['issue_us']:>6.2f} "
+              f"{r['drain_us']:>6.2f} {r['epilogue2_us']:>6.2f}")
     tot = sum(r['us'] * r['count'] for r in rows)
     bnd = sum(r['bound_us'] * r['count'] for r in rows)
     print(f"step total: {tot / 1e3:.3f} ms of back-to-back launches, tensor-rate bound {bnd / 1e3:.3f} ms")
