@@ -20,12 +20,12 @@ from ._lib import MOS_SEG_ROWS, MOS_SEG_TRANSPOSED
 
 BF16 = torch.bfloat16       # weights (and the training engine's activations)
 F16 = torch.float16
-# split-K GEMMs finalize in-kernel (mos_gemm_args.tile_counters); MOS_SPLITK_FUSED=0 restores the separate
-# mos_splitk_finalize launch (A/B timing)
+# split-K GEMMs are finalized by a separate mos_splitk_finalize launch; MOS_SPLITK_FUSED=1 (off by default) has the GEMM
+# finalize in-kernel instead (mos_gemm_args.tile_counters), with the same summation order and bit-identical results
 FUSED_SPLITK = os.environ.get('MOS_SPLITK_FUSED', '0') == '1'
-# every GEMM of the step stages the NEXT GEMM's weight matrix in L2 while it runs (mos_gemm_args.prefetch_ptr): the step
-# streams 1.7 GB of weights through a mostly idle HBM, and the 50 MB L2 of an H100 holds any single layer (at most 48 MB
-# is staged).  MOS_L2_PREFETCH=0/1.
+# MOS_L2_PREFETCH=1 (off by default): every GEMM of the step stages the NEXT GEMM's weight matrix in L2 while it runs
+# (mos_gemm_args.prefetch_ptr): the step streams 1.7 GB of weights through a mostly idle HBM, and the 50 MB L2 of an H100
+# holds any single layer (at most 48 MB is staged).
 L2_PREFETCH = os.environ.get('MOS_L2_PREFETCH', '0') == '1'
 L2_PREFETCH_MAX_BYTES = 48 << 20
 SPLITK_MIN_KB = int(os.environ.get('MOS_SPLITK_MIN_KB', '8'))      # fewest 64-deep k-blocks a split-K slice may get
