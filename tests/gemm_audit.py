@@ -425,7 +425,7 @@ class _Storages:
 def _site():
     for fr in reversed(traceback.extract_stack()[:-1]):
         f = fr.filename.replace('\\', '/')
-        if f.endswith(('/ops.py', '/gemm_audit.py')) or fr.name in ('gemm', '_audited'):
+        if f.endswith(('/ops.py', '/gemm_audit.py', '/attention_audit.py')) or fr.name in ('gemm', '_audited'):
             continue
         return f"{f.rsplit('/', 1)[-1]}:{fr.lineno}"
     return '?'

@@ -27,6 +27,7 @@ if __name__ == '__main__':
     _root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     sys.path[:0] = [_root, os.path.join(_root, 'mix-of-show_b200'), os.path.dirname(os.path.abspath(__file__))]
 
+import engine_walks as walks  # noqa: E402
 import gemm_audit as ga  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -112,27 +113,11 @@ def _audited(fn):
 
 @pytest.fixture(scope='module')
 def sd15():
-    from oracle import inject
-    from oracle import unet as ou
-    unet = ou.build_unet(0, None)
-    inject.install_edlora_processors(unet)
-    return unet, {k: v.clone() for k, v in unet.state_dict().items()}
+    return walks.sd15_pair()
 
 
 def walk_sample64(sd15_pair, stats):
-    from mos_b200.engine import UNetEngine, ehs_to_layer_major
-    from oracle import inject
-    unet, sd = sd15_pair
-    lora = inject.random_lora_state(unet, seed=10)
-    g = torch.Generator().manual_seed(1)
-    lat = torch.randn(1, 4, 64, 64, generator=g)
-    ehs = torch.randn(2, 16, 77, 768, generator=torch.Generator().manual_seed(2))
-    eng = UNetEngine(sd, 2, 64, 64, lora=lora, lora_alpha=1.0, use_graph=False)
-    with ga.Recorder(stats):
-        eps = eng.forward(torch.cat([lat, lat]).cuda(), torch.tensor([981.0, 981.0]).cuda(),
-                          ehs_to_layer_major(ehs.cuda())).clone()
-        torch.cuda.synchronize()
-    return eps
+    return walks.sample_64(sd15_pair, lambda: ga.Recorder(stats))
 
 
 def test_sample_64(cuda, sd15):
@@ -140,65 +125,15 @@ def test_sample_64(cuda, sd15):
 
 
 def test_sample_96x192_whole_block(cuda, sd15):
-    from mos_b200.engine import UNetEngine, ehs_to_layer_major
-    from oracle import inject
-    unet, sd = sd15
-    lora = inject.random_lora_state(unet, seed=11, where='Transformer2DModel', up_std=0.05)
-    g = torch.Generator().manual_seed(3)
-    lat = torch.randn(2, 4, 96, 192, generator=g)
-    ehs = torch.randn(2, 16, 77, 768, generator=g)
-    eng = UNetEngine(sd, 2, 96, 192, lora=lora, lora_alpha=0.8, use_graph=False)
-    _audited(lambda: eng.forward(lat.cuda(), torch.tensor([501.0, 501.0]).cuda(), ehs_to_layer_major(ehs.cuda())))
+    walks.sample_96x192_whole_block(sd15, lambda: ga.Recorder(STATS))
 
 
 def test_train_sd15_channels_whole_block(cuda):
-    from mos_b200.engine import ehs_to_layer_major
-    from mos_b200.train_engine import TrainEngine
-    from oracle import inject
-    from oracle import unet as ou
-    cfg = dict(block_out_channels=(320, 640, 1280, 1280), layers_per_block=1)
-    ref = ou.build_unet(0, cfg)
-    lora = inject.random_lora_state(ref, seed=10, where='Transformer2DModel')
-    sd = {k: v.detach().clone() for k, v in ref.state_dict().items()}
-    g = torch.Generator().manual_seed(5)
-    B, H = 2, 16
-    x0, noise = torch.randn(B, 4, H, H, generator=g), torch.randn(B, 4, H, H, generator=g)
-    eng = TrainEngine(sd, B, H, H, lora=lora, attn_reg_weight=None, where='Transformer2DModel',
-                      block_out=cfg['block_out_channels'], layers=1, use_graph=False)
-    n_x = len(eng.xattn_names)
-    ehs = torch.randn(B, n_x, 77, 768, generator=g)
-    _audited(lambda: eng.forward_backward(x0.cuda(), noise.cuda(), torch.tensor([77, 640]).cuda(),
-                                          ehs_to_layer_major(ehs.cuda(), n_x), torch.ones(B, 1, H, H).cuda()))
+    walks.train_sd15_channels_whole_block(lambda: ga.Recorder(STATS))
 
 
 def test_clip_text_and_train(cuda):
-    from transformers import CLIPTextConfig, CLIPTextModel
-    from mos_b200.clip_engine import CLIPTextEngine
-    from mos_b200.clip_train_engine import CLIPTrainEngine
-    from oracle import inject
-    cfg = CLIPTextConfig(vocab_size=49408 + 32, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
-                         num_attention_heads=12, max_position_embeddings=77)
-    torch.manual_seed(0)
-    model = CLIPTextModel(cfg).eval()
-    sd = {k: v.clone() for k, v in model.state_dict().items()}
-    g = torch.Generator().manual_seed(3)
-    ids = torch.randint(0, 49407, (16, 77), generator=g)
-    ids[:, 0] = 49406
-    ids[:, 9:] = 49407
-    concept_ids = list(range(49408, 49408 + 32))
-    ids[:, 4] = torch.tensor(concept_ids[:16])
-    ids[:, 5] = torch.tensor(concept_ids[16:])
-    lora_a = inject.random_lora_state(model, seed=7, where='CLIPAttention', up_std=0.05)
-    eng = CLIPTextEngine(sd, 16, lora=lora_a, lora_alpha=0.8)
-    _audited(lambda: eng(ids))
-    lora_l = inject.random_lora_state(model, seed=8, where='CLIPEncoderLayer', up_std=0.05)
-    tr = CLIPTrainEngine(sd, 16, lora=lora_l, lora_alpha=0.8, concept_token_ids=concept_ids)
-    dy = (torch.randn(16 * 77, 768, generator=g) * 0.05).to(cuda).to(torch.bfloat16)
-
-    def fwd_bwd():
-        tr.forward_train(ids)
-        tr.backward(dy)
-    _audited(fwd_bwd)
+    walks.clip_text_and_train(lambda: ga.Recorder(STATS), cuda)
 
 
 def test_vae_512(cuda):
@@ -257,12 +192,8 @@ def test_coverage_table(cuda):
 
 if __name__ == '__main__':
     torch.backends.cuda.matmul.allow_tf32 = False
-    from oracle import inject
-    from oracle import unet as ou
-    _unet = ou.build_unet(0, None)
-    inject.install_edlora_processors(_unet)
     _stats = ga.Stats()
-    _eps = walk_sample64((_unet, {k: v.clone() for k, v in _unet.state_dict().items()}), _stats)
+    _eps = walk_sample64(walks.sd15_pair(), _stats)
     torch.save(_eps.cpu(), os.path.join(sys.argv[1], 'eps.pt'))
     with open(os.path.join(sys.argv[1], 'stats.json'), 'w') as f:
         json.dump({'rows': _stats.rows, 'failures': _stats.failures}, f)
