@@ -14,20 +14,28 @@ namespace mos {
 
 constexpr int GN_GROUPS = 32;
 
-// The statistics of a (sample, group) are accumulated about a pivot p, the group's first element in the sample's first
-// row: sums of (x - p) and (x - p)^2, then mean = p + S/n and var = Q/n - (S/n)^2.  Raw sums of x and x^2 would lose the
-// variance to cancellation once the group's mean is large against its spread (E[x^2] - mean^2 in fp32).  Every chunk and
-// every CTA of a cluster reads the same pivot, so the partials still add up in a fixed order.
+// GroupNorm statistics are centred.  Raw sums of x and x^2 lose the variance to cancellation once the group's mean is large
+// against its spread (E[x^2] - mean^2 in fp32), and sums about any one element p lose it once that element lies far from
+// the group's mean (the error grows with ((p - mean) / std)^2; the top-left pixel, where the zero padding of 3x3
+// convolutions leaves its mark, can lie up to sqrt(n) std away).  So:
+//  - the cluster kernel sums x - p and (x - p)^2 about p, the group's first element in the sample's first row (which keeps
+//    constant groups exact).  When p lies more than 4 std from the mean, it sums x - m and (x - m)^2 about that mean m
+//    in a second pass over the slab it holds in shared memory;
+//  - the statistics kernel of the fallback and the backward keeps a running (mean, M2) per thread and channel (Welford)
+//    and writes one (mean, M2) per (chunk, group); gn_merge_chunks merges the chunks about the first chunk's mean and
+//    adds their centred terms.
+// Every merge runs in a fixed order, so the statistics are bitwise reproducible.
+
 template <bool F16>
 __device__ __forceinline__ float gn_pivot(const __nv_bfloat16* x, long long ldx, int b, int HW, int c0) {
   return ld16<F16>(x + (long long)b * HW * ldx + c0);
 }
 
-// partial[b][chunk][g][2] = (sum, sumsq) of (x - pivot_g) over rows [chunk*rows_per_chunk, ...) of batch b
+// partial[b][chunk][g][2] = (mean, M2 = sum of (x - mean)^2) over rows [chunk*rows_per_chunk, ...) of batch b
 template <bool F16>
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int C,
                                 int rows_per_chunk, float* __restrict__ partial) {
-  extern __shared__ float red[];  // [blockDim][16]: per-thread channel sums / sums of squares
+  extern __shared__ float red[];  // [blockDim][16]: per-thread channel means / M2
   pdl_wait();
   pdl_launch_dependents();
   const int oct = C / 8, cpg = C / GN_GROUPS;
@@ -35,12 +43,10 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long l
   const int lanes = blockDim.x / oct;  // row lanes; blockDim is a multiple of oct
   const int o = threadIdx.x % oct, rl = threadIdx.x / oct;
   const int r0 = chunk * rows_per_chunk, r1 = min(HW, r0 + rows_per_chunk);
-  float s[8], q[8], p[8];
+  float m[8], m2[8];   // Welford: running mean and sum of squared deviations of the thread's rows, per channel
+  int cnt = 0;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    s[i] = q[i] = 0.f;
-    p[i] = gn_pivot<F16>(x, ldx, b, HW, (o * 8 + i) / cpg * cpg);
-  }
+  for (int i = 0; i < 8; ++i) m[i] = m2[i] = 0.f;
   const __nv_bfloat16* base = x + ((long long)b * HW) * ldx + o * 8;
   for (int rb = r0 + rl; rb < r1; rb += 4 * lanes) {
     uint4 u4[4];   // four independent 16-byte loads in flight per thread
@@ -52,37 +58,80 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long l
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (rb + k * lanes >= r1) continue;
+      const float inv = __frcp_rn((float)(++cnt));
       const uint32_t w[4] = {u4[k].x, u4[k].y, u4[k].z, u4[k].w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 f = unpack16x2<F16>(w[i]);
-        const float d0 = f.x - p[2 * i], d1 = f.y - p[2 * i + 1];
-        s[2 * i] += d0;
-        q[2 * i] += d0 * d0;
-        s[2 * i + 1] += d1;
-        q[2 * i + 1] += d1 * d1;
+        const float d0 = f.x - m[2 * i], d1 = f.y - m[2 * i + 1];
+        m[2 * i] = fmaf(d0, inv, m[2 * i]);
+        m[2 * i + 1] = fmaf(d1, inv, m[2 * i + 1]);
+        m2[2 * i] = fmaf(d0, f.x - m[2 * i], m2[2 * i]);
+        m2[2 * i + 1] = fmaf(d1, f.y - m[2 * i + 1], m2[2 * i + 1]);
       }
     }
   }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    red[threadIdx.x * 16 + i] = s[i];
-    red[threadIdx.x * 16 + 8 + i] = q[i];
+    red[threadIdx.x * 16 + i] = m[i];
+    red[threadIdx.x * 16 + 8 + i] = m2[i];
   }
   __syncthreads();
-  if (threadIdx.x < GN_GROUPS) {  // fixed summation order -> bitwise reproducible statistics
-    const int g = threadIdx.x;
-    float gs = 0.f, gq = 0.f;
+  if (threadIdx.x < GN_GROUPS) {  // fixed order -> bitwise reproducible statistics
+    // Row lane l holds the (mean, M2) of rows r0 + l + j * lanes: q0 or q0 + 1 of them.  The group's mean is the first
+    // partial's mean plus the weighted mean of the differences to it; M2 = sum of (M2 + rows * (mean_l,c - mean)^2).
+    const int g = threadIdx.x, rows = r1 - r0, q0 = rows / lanes, rem = rows - q0 * lanes;
+    const float m0 = red[((g * cpg) >> 3) * 16 + ((g * cpg) & 7)];   // lane 0 holds at least one row
+    float s = 0.f;
+    for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
+      for (int l = 0; l < lanes; ++l) s = fmaf((float)(q0 + (l < rem)), red[(l * oct + (c >> 3)) * 16 + (c & 7)] - m0, s);
+    }
+    const float mu = m0 + s / ((float)rows * (float)cpg);
+    float q = 0.f;
     for (int c = g * cpg; c < (g + 1) * cpg; ++c) {
       for (int l = 0; l < lanes; ++l) {
         const float* t = red + (l * oct + (c >> 3)) * 16 + (c & 7);
-        gs += t[0];
-        gq += t[8];
+        const float d = t[0] - mu;
+        q += fmaf((float)(q0 + (l < rem)) * d, d, t[8]);
       }
     }
     float* dst = partial + (((long long)b * nchunks + chunk) * GN_GROUPS + g) * 2;
-    dst[0] = gs;
-    dst[1] = gq;
+    dst[0] = mu;
+    dst[1] = q;
+  }
+}
+
+// mean / rstd of the (sample, group) pairs of batch b from the per-chunk (mean, M2) of gn_stats_kernel, on threads
+// [0, 128): 4 threads per group over strided chunks, then a shuffle tree (fixed order).  The mean is the first chunk's
+// mean plus the row-weighted mean of the differences to it, which keeps a constant group exact; the variance adds each
+// chunk's M2 and its centred term rows * cpg * (mean_c - mean)^2.
+__device__ __forceinline__ void gn_merge_chunks(const float* __restrict__ partial, int nchunks, int rows_per_chunk,
+                                                int b, int HW, int cpg, float eps, float* mean, float* rstd) {
+  if (threadIdx.x < GN_GROUPS * 4) {
+    const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
+    const float2* pg = reinterpret_cast<const float2*>(partial) + (long long)b * nchunks * GN_GROUPS + g;
+    const float m0 = __ldg(pg).x;
+    float s = 0.f;
+    for (int c = sub; c < nchunks; c += 4) {
+      const float rows = (float)(min(HW, (c + 1) * rows_per_chunk) - c * rows_per_chunk);
+      s = fmaf(rows, __ldg(pg + (long long)c * GN_GROUPS).x - m0, s);
+    }
+#pragma unroll
+    for (int d = 2; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
+    const float mu = m0 + s / (float)HW;
+    float q = 0.f;
+    for (int c = sub; c < nchunks; c += 4) {
+      const float n = (float)(min(HW, (c + 1) * rows_per_chunk) - c * rows_per_chunk) * (float)cpg;
+      const float2 v = __ldg(pg + (long long)c * GN_GROUPS);
+      const float d = v.x - mu;
+      q += fmaf(n * d, d, v.y);
+    }
+#pragma unroll
+    for (int d = 2; d > 0; d >>= 1) q += __shfl_xor_sync(0xffffffffu, q, d);
+    if (sub == 0) {
+      mean[g] = mu;
+      rstd[g] = rsqrtf(fmaxf(q / ((float)HW * (float)cpg), 0.f) + eps);
+    }
   }
 }
 
@@ -96,27 +145,7 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
   pdl_launch_dependents();
   const int b = blockIdx.y;
   const int cpg = C / GN_GROUPS;
-  if (threadIdx.x < GN_GROUPS * 4) {   // blockDim >= 160 always
-    // 4 threads per group sum the per-chunk partials (fixed order -> reproducible), then a shuffle tree
-    const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
-    float s = 0.f, q = 0.f;
-    for (int c = sub; c < nchunks; c += 4) {
-      const float2 v = __ldg(reinterpret_cast<const float2*>(partial + (((long long)b * nchunks + c) * GN_GROUPS + g) * 2));
-      s += v.x;
-      q += v.y;
-    }
-#pragma unroll
-    for (int d = 2; d > 0; d >>= 1) {
-      s += __shfl_xor_sync(0xffffffffu, s, d);
-      q += __shfl_xor_sync(0xffffffffu, q, d);
-    }
-    if (sub == 0) {
-      const float n = (float)HW * (float)cpg;
-      const float d = s / n;    // mean - pivot
-      mean[g] = gn_pivot<F16>(x, ldx, b, HW, g * cpg) + d;
-      rstd[g] = rsqrtf(fmaxf(q / n - d * d, 0.f) + eps);
-    }
-  }
+  gn_merge_chunks(partial, nchunks, rows_per_block, b, HW, cpg, eps, mean, rstd);   // blockDim >= 160 always
   __syncthreads();
   const int oct = C / 8;
   const int lanes = blockDim.x / oct;
@@ -242,10 +271,10 @@ __global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long 
 // ---------------------------------------------------------------------------------------------- one-pass GroupNorm
 // GroupNorm(+SiLU) in ONE launch with ONE read of x: a thread-block cluster of k CTAs (k = 1, 2, 4, 8) owns one
 // (sample, group) pair.  Each CTA streams its rows of the group's channel slab (cpg = C / 32 channels, 20..160 bytes
-// per row) into shared memory while accumulating sum / sum of squares, the k partial pairs are exchanged through
-// distributed shared memory (every CTA stores its pair into every peer's table, one cluster barrier, everybody adds the
-// table in rank order: fixed order -> bitwise reproducible and identical in all CTAs), and the slab is normalised out of
-// shared memory.  Replaces gn_stats + gn_apply (two launches, two reads of x, a partial-statistics round trip through
+// per row) into shared memory while accumulating sum / sum of squares about the pivot, the k partial pairs are exchanged
+// through distributed shared memory (gn_cluster_sum: fixed order -> bitwise reproducible and identical in all CTAs), an
+// outlying pivot triggers a second, centred pass over the slab (exchanged the same way), and the slab is normalised out
+// of shared memory.  Replaces gn_stats + gn_apply (two launches, two reads of x, a partial-statistics round trip through
 // global memory); those remain as the fallback for slabs that do not fit 8 x 200 KB.
 // Thread layout: thread = (row lane, VEC-element column word); blockDim = lanes * (cpg / VEC), so the column word - and
 // with it gamma / beta - is fixed per thread and no index division happens inside the loops; every thread re-reads only
@@ -259,6 +288,46 @@ __device__ __forceinline__ void st_cluster_f32x2(uint32_t raddr, float a, float 
   asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(raddr), "f"(a), "f"(b) : "memory");
 }
 
+// (s, q) summed over the CTA's threads, then over the cluster's k CTAs in rank order through `table` (every CTA stores its
+// pair into every peer's table, one cluster barrier): the same bits in every thread of every CTA.  Called by all threads.
+// A table serves one call only, since a peer may still be reading it when this CTA reaches the next call.
+__device__ __forceinline__ float2 gn_cluster_sum(float s, float q, float (*wred)[2], float2* table, int k, int rank,
+                                                 bool wait_peers) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    s += __shfl_xor_sync(0xffffffffu, s, d);
+    q += __shfl_xor_sync(0xffffffffu, q, d);
+  }
+  const int warp = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
+  if ((threadIdx.x & 31) == 0) {
+    wred[warp][0] = s;
+    wred[warp][1] = q;
+  }
+  __syncthreads();
+  if (wait_peers && k > 1) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");   // all peers have started
+  if (threadIdx.x == 0) {
+    float ts = 0.f, tq = 0.f;
+    for (int w = 0; w < nwarps; ++w) {
+      ts += wred[w][0];
+      tq += wred[w][1];
+    }
+    if (k > 1) {
+      const uint32_t slot = smem_u32(&table[rank]);
+      for (int peer = 0; peer < k; ++peer) st_cluster_f32x2(mapa_u32(slot, (uint32_t)peer), ts, tq);
+    } else {
+      table[0] = make_float2(ts, tq);
+    }
+  }
+  if (k > 1) cluster_sync_all();     // release / acquire at cluster scope: the peers' table stores are visible
+  else __syncthreads();
+  float2 t = make_float2(0.f, 0.f);
+  for (int i = 0; i < k; ++i) {
+    t.x += table[i].x;
+    t.y += table[i].y;
+  }
+  return t;
+}
+
 template <bool F16, int VEC>   // VEC = 16-bit elements per load / store: 4 (cpg % 4 == 0) or 2
 __global__ void __launch_bounds__(256)
 gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int C, int rows_per_cta, int k, int lanes,
@@ -266,8 +335,7 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
                 __nv_bfloat16* __restrict__ y, long long ldy) {
   extern __shared__ __align__(16) uint8_t gsm[];
   __shared__ float wred[8][2];
-  __shared__ float2 table[8];       // per-CTA partial (sum, sumsq), filled by the peers through DSMEM
-  __shared__ float stat[2];
+  __shared__ float2 table[2][8];    // per-CTA partials of the two passes, filled by the peers through DSMEM
   // Distributed shared memory may only be touched once every CTA of the cluster is known to be running: arrive here, wait
   // right before the first remote store (the loads and the local reduction in between hide the barrier latency).
   if (k > 1) asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -315,47 +383,38 @@ gn_group_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int 
       }
     }
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) {
-    s += __shfl_xor_sync(0xffffffffu, s, d);
-    q += __shfl_xor_sync(0xffffffffu, q, d);
-  }
-  const int warp = threadIdx.x >> 5, nwarps = (blockDim.x + 31) >> 5;
-  if ((threadIdx.x & 31) == 0) {
-    wred[warp][0] = s;
-    wred[warp][1] = q;
-  }
-  __syncthreads();
-  if (k > 1) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");   // all peers have started
-  if (threadIdx.x == 0) {
-    float ts = 0.f, tq = 0.f;
-    for (int w = 0; w < nwarps; ++w) {
-      ts += wred[w][0];
-      tq += wred[w][1];
+  const float n = (float)HW * (float)cpg;
+  float2 t = gn_cluster_sum(s, q, wred, table[0], k, rank, true);
+  float d = t.x / n;    // mean - pivot
+  float mean = p + d, var = t.y / n - d * d;
+  // The cancellation error of var grows with ((p - mean) / std)^2.  Beyond 4 std (an outlying pivot element) sum again,
+  // about the mean, over the slab words this thread stored.  Every CTA of the cluster holds the same t: the branch and
+  // the second exchange are uniform across the cluster.
+  if (d * d > 16.f * var) {
+    float s2 = 0.f, q2 = 0.f;
+    if (rl < lanes) {
+      for (int r = r0 + rl; r < r1; r += lanes) {
+        const word_t w = slab[(r - r0) * vpr + v];
+        if constexpr (VEC == 4) {
+          const float2 f0 = unpack16x2<F16>(w.x), f1 = unpack16x2<F16>(w.y);
+          const float d0 = f0.x - mean, d1 = f0.y - mean, d2 = f1.x - mean, d3 = f1.y - mean;
+          s2 += (d0 + d1) + (d2 + d3);
+          q2 += (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+        } else {
+          const float2 f0 = unpack16x2<F16>(w);
+          const float d0 = f0.x - mean, d1 = f0.y - mean;
+          s2 += d0 + d1;
+          q2 += d0 * d0 + d1 * d1;
+        }
+      }
     }
-    if (k > 1) {
-      const uint32_t slot = smem_u32(&table[rank]);
-      for (int peer = 0; peer < k; ++peer) st_cluster_f32x2(mapa_u32(slot, (uint32_t)peer), ts, tq);
-    } else {
-      table[0] = make_float2(ts, tq);
-    }
+    t = gn_cluster_sum(s2, q2, wred, table[1], k, rank, false);
+    d = t.x / n;
+    mean += d;
+    var = t.y / n - d * d;
   }
-  if (k > 1) cluster_sync_all();     // release / acquire at cluster scope: the peers' table stores are visible
-  else __syncthreads();
-  if (threadIdx.x == 0) {
-    float ts = 0.f, tq = 0.f;
-    for (int i = 0; i < k; ++i) {
-      ts += table[i].x;
-      tq += table[i].y;
-    }
-    const float n = (float)HW * (float)cpg;
-    const float d = ts / n;    // mean - pivot
-    stat[0] = p + d;
-    stat[1] = rsqrtf(fmaxf(tq / n - d * d, 0.f) + eps);
-  }
-  __syncthreads();
+  const float rstd = rsqrtf(fmaxf(var, 0.f) + eps);
   if (rl >= lanes) return;
-  const float mean = stat[0], rstd = stat[1];
   float sc[VEC], sh[VEC];   // y = (x - mean) * sc + sh, as in gn_apply_kernel
 #pragma unroll
   for (int i = 0; i < VEC; ++i) {
@@ -403,32 +462,6 @@ __device__ __forceinline__ float silu_grad(float z) {
   return sg * (1.0f + z * (1.0f - sg));
 }
 
-// mean / rstd of the (sample, group) pairs from the partials of gn_stats_kernel<false> (bf16 x: training)
-__device__ __forceinline__ void gn_load_stats(const __nv_bfloat16* __restrict__ x, long long ldx,
-                                              const float* __restrict__ partial, int nchunks, int b, int HW, int cpg,
-                                              float eps, float* mean, float* rstd) {
-  if (threadIdx.x < GN_GROUPS * 4) {
-    const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
-    float s = 0.f, q = 0.f;
-    for (int c = sub; c < nchunks; c += 4) {
-      const float2 v = __ldg(reinterpret_cast<const float2*>(partial + (((long long)b * nchunks + c) * GN_GROUPS + g) * 2));
-      s += v.x;
-      q += v.y;
-    }
-#pragma unroll
-    for (int d = 2; d > 0; d >>= 1) {
-      s += __shfl_xor_sync(0xffffffffu, s, d);
-      q += __shfl_xor_sync(0xffffffffu, q, d);
-    }
-    if (sub == 0) {
-      const float n = (float)HW * (float)cpg;
-      const float d = s / n;    // mean - pivot
-      mean[g] = gn_pivot<false>(x, ldx, b, HW, g * cpg) + d;
-      rstd[g] = rsqrtf(fmaxf(q / n - d * d, 0.f) + eps);
-    }
-  }
-}
-
 // partial2[b][chunk][g][2] = (sum dz*gamma, sum dz*gamma*xhat)
 __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, long long ldx,
                                      const __nv_bfloat16* __restrict__ dy, long long lddy, int HW, int C,
@@ -441,7 +474,7 @@ __global__ void gn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ x, long l
   pdl_launch_dependents();
   const int b = blockIdx.y, chunk = blockIdx.x, nchunks = gridDim.x;
   const int cpg = C / GN_GROUPS;
-  gn_load_stats(x, ldx, partial, nchunks, b, HW, cpg, eps, mean, rstd);
+  gn_merge_chunks(partial, nchunks, rows_per_chunk, b, HW, cpg, eps, mean, rstd);   // of gn_stats_kernel<false>
   __syncthreads();
   const int oct = C / 8;
   const int lanes = blockDim.x / oct;
@@ -512,7 +545,7 @@ __global__ void gn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ x, long lo
   pdl_launch_dependents();
   const int b = blockIdx.y, nchunks = gridDim.x;
   const int cpg = C / GN_GROUPS;
-  gn_load_stats(x, ldx, partial, nchunks, b, HW, cpg, eps, mean, rstd);
+  gn_merge_chunks(partial, nchunks, rows_per_chunk, b, HW, cpg, eps, mean, rstd);   // of gn_stats_kernel<false>
   if (threadIdx.x < GN_GROUPS * 4) {
     const int g = threadIdx.x >> 2, sub = threadIdx.x & 3;
     float s = 0.f, q = 0.f;

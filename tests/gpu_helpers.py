@@ -81,6 +81,40 @@ def gn_path(B, HW, C, ldx, ldy, sms=None):
     return 'fallback'
 
 
+def plant_outlier(x, C, layout, K, seed):
+    """x [B, HW, ld] with NaN pad columns; returns a copy in which the group's first element of row 0 (layout 'pivot'), or
+    all C channels of row 0 (layout 'corner': the top-left pixel, where the zero padding of 3x3 convolutions leaves its
+    mark), lies K x the group's std away from the group's mean, with a random sign per (sample, group).  K = 'max' is
+    sqrt(n) / 2 for the group size n = HW * C / 32: one element can lie at most sqrt(n - 1) std from its group's mean.
+    Also returns the boolean mask of the planted elements over [B, HW, C]."""
+    B, HW = x.shape[:2]
+    cpg = C // 32
+    if K == 'max':
+        K = (HW * cpg) ** 0.5 / 2
+    g = torch.Generator(device='cpu').manual_seed(seed)
+    sign = torch.where(torch.rand(B, 1, 32, 1, generator=g) < 0.5, -1.0, 1.0).to(x.device)
+    body = x[..., :C].double().view(B, HW, 32, cpg)
+    mean = body.mean(dim=(1, 3), keepdim=True)
+    std = body.std(dim=(1, 3), keepdim=True)
+    mask = torch.zeros(B, HW, 32, cpg, dtype=torch.bool, device=x.device)
+    if layout == 'pivot':
+        mask[:, 0, :, 0] = True
+    else:
+        mask[:, 0] = True
+    planted = torch.where(mask, mean + sign * K * std, body)
+    out = x.clone()
+    out[..., :C] = planted.view(B, HW, C).to(x.dtype)
+    return out, mask.view(B, HW, C)
+
+
+def worst_group_rel_l2(y, ref, C):
+    """the largest rel-L2 over the (sample, group) pairs of [B, HW, C] outputs"""
+    B, HW = y.shape[:2]
+    d = (y.double() - ref.double()).view(B, HW, 32, C // 32)
+    r = ref.double().view(B, HW, 32, C // 32)
+    return (d.norm(dim=(1, 3)) / r.norm(dim=(1, 3)).clamp_min(1e-300)).max().item()
+
+
 def pack_rows(t, dp):
     """[B, H, n, d] -> the zero-padded head-split row layout [B*H, n, dp]"""
     B, H, n, d = t.shape

@@ -58,8 +58,10 @@ def test_layernorm_bwd_pitched_offset(cuda, off):
 
 # off: group mean / std (a per-(sample, group) offset); pad: extra columns of dy, dx and add (lddy = lddx = ldadd = C + pad);
 # ws: workspace floats (B * 128 holds one chunk of both partial tables)
-def _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off=0, pad=0, ws=1 << 18):
-    from gpu_helpers import canary, untouched, window_mask
+# outlier: (layout, K) of gpu_helpers.plant_outlier: the group's first element of row 0, or all of row 0, K std from its
+# mean
+def _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off=0, pad=0, ws=1 << 18, outlier=None):
+    from gpu_helpers import canary, plant_outlier, untouched, window_mask, worst_group_rel_l2
     from mos_b200 import ops
     g = torch.Generator(device='cpu').manual_seed(5)
     sign = torch.where(torch.rand(B, 1, 32, 1, generator=g) < 0.5, -1.0, 1.0)
@@ -67,6 +69,8 @@ def _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off=0, pad=0, ws=1 << 18):
     buf = mk((B, HW, ld), cuda, 1.5, 1).float() + 0.3
     buf[..., :C] += shift
     buf = buf.to(BF)
+    if outlier is not None:
+        buf, _ = plant_outlier(buf, C, *outlier, seed=6)
     x = buf[..., :C]
     ldp = C + pad
     dyb = torch.full((B, HW, ldp), float('nan'), device=cuda, dtype=BF)
@@ -86,16 +90,25 @@ def _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off=0, pad=0, ws=1 << 18):
     ops.groupnorm_bwd(x, dy, gamma, beta, dx, wsb, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld, lddy=ldp, lddx=ldp)
     assert untouched(dxb, window_mask(dxb, slice(0, B * HW), slice(0, C)))
     e = rel_l2(dx, ref)
+    # the planted element must not hide a bad group behind the global norm; without add, so that add does not dilute it
+    e_group = worst_group_rel_l2(dx, ref, C) if outlier is not None else None
     ops.groupnorm_bwd(x, dy, gamma, beta, dx, wsb, B=B, HW=HW, C=C, eps=1e-5, silu=silu, ldx=ld, lddy=ldp, lddx=ldp,
                       add=add, ldadd=ldp)
     e_add = rel_l2(dx, ref + add.double())
-    print(f'GN bwd B={B} HW={HW} C={C} offset {off} pad {pad} ws {ws}: rel-L2 {e:.2e}, with add {e_add:.2e}')
+    print(f'GN bwd B={B} HW={HW} C={C} offset {off} pad {pad} ws {ws} outlier {outlier}: rel-L2 {e:.2e}, '
+          f'with add {e_add:.2e}')
     assert e < 5e-3 and e_add < 5e-3
+    if outlier is not None:
+        e_group_add = worst_group_rel_l2(dx, ref + add.double(), C)
+        print(f'  worst group rel-L2 {e_group:.2e}, with add {e_group_add:.2e}')
+        assert e_group < 5e-3 and e_group_add < 5e-3
 
 
-@pytest.mark.parametrize('B,HW,C,ld,silu', [(2, 4096, 320, 320, True), (2, 1024, 1920, 1920, True),
-                                             (2, 256, 640, 1280, False), (3, 64, 1280, 1280, True),
-                                             (1, 1024, 960, 960, True)])
+GN_BWD_SHAPES = [(2, 4096, 320, 320, True), (2, 1024, 1920, 1920, True), (2, 256, 640, 1280, False),
+                 (3, 64, 1280, 1280, True), (1, 1024, 960, 960, True)]
+
+
+@pytest.mark.parametrize('B,HW,C,ld,silu', GN_BWD_SHAPES)
 def test_groupnorm_bwd(cuda, B, HW, C, ld, silu):
     _check_groupnorm_bwd(cuda, B, HW, C, ld, silu)
 
@@ -107,6 +120,22 @@ def test_groupnorm_bwd(cuda, B, HW, C, ld, silu):
 def test_groupnorm_bwd_offset_pitched(cuda, B, HW, C, ld, silu, off, pad, ws):
     """group means up to 100 x their std, dy / dx / add pitches above C, and a one-chunk workspace"""
     _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, off, pad, ws)
+
+
+@pytest.mark.parametrize('K', [30, 100, 300, 'max'])
+@pytest.mark.parametrize('layout', ['pivot', 'corner'])
+@pytest.mark.parametrize('B,HW,C,ld,silu', GN_BWD_SHAPES)
+def test_groupnorm_bwd_outlier(cuda, B, HW, C, ld, silu, layout, K):
+    """the group's first element of row 0, or the whole first pixel, K x the group's std from its mean: the recomputed
+    statistics must not lose the variance to cancellation against it"""
+    _check_groupnorm_bwd(cuda, B, HW, C, ld, silu, outlier=(layout, K))
+
+
+@pytest.mark.parametrize('K', [30, 300, 'max'])
+@pytest.mark.parametrize('layout', ['pivot', 'corner'])
+def test_groupnorm_bwd_outlier_one_chunk(cuda, layout, K):
+    """a workspace of one chunk per sample: each statistics thread runs over HW / lanes = 512 rows, the outlier first"""
+    _check_groupnorm_bwd(cuda, 2, 4096, 320, 320, True, ws=2 * 128, outlier=(layout, K))
 
 
 def test_geglu_fwd_bwd(cuda):

@@ -20,7 +20,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from gpu_helpers import canary, gn_path, num_sms, rel_l2, rup, same_bits, untouched, window_mask
+from gpu_helpers import (canary, gn_path, num_sms, plant_outlier, rel_l2, rup, same_bits, untouched, window_mask,
+                         worst_group_rel_l2)
 
 pytestmark = pytest.mark.gpu
 BF, H16 = torch.bfloat16, torch.float16
@@ -181,6 +182,29 @@ def test_groupnorm_offset(cuda, gn_mode, shape, dtype, ratio):
     e = rel_l2(y, _reference(x, C, gamma, beta, eps, True))
     print(f'GN offset {ratio:>3} {"bf16" if dtype == BF else "fp16"} {_label(shape[:6])} '
           f'[{gn_mode}: {_expected(gn_mode, B, HW, C, ldx, ldy)}] rel-L2 {e:.2e}')
+    assert e < TOL[dtype]
+
+
+OUTLIER_SHAPES = [('unet', 2, 4096, 320, 320, 320, 1e-5), ('vae', 1, 262144, 128, 160, 128, 1e-6),
+                  ('vae', 2, 65536, 256, 320, 256, 1e-6)]
+
+
+@pytest.mark.parametrize('K', [30, 100, 300, 'max'])
+@pytest.mark.parametrize('layout', ['pivot', 'corner'])
+@pytest.mark.parametrize('dtype', [BF, H16], ids=['bf16', 'fp16'])
+@pytest.mark.parametrize('shape', OUTLIER_SHAPES, ids=[_label(s[:6]) for s in OUTLIER_SHAPES])
+def test_groupnorm_outlier_pivot(cuda, gn_mode, shape, dtype, layout, K):
+    """The element the statistics used to be pivoted on (the group's first element in the sample's first row), or the
+    whole first pixel, lies far from its group's mean: the variance must not be lost to cancellation against it.  Held to
+    the offset bounds in every (sample, group), not only over the whole tensor."""
+    name, B, HW, C, ldx, ldy, eps = shape
+    x, _ = plant_outlier(_input(B, HW, C, ldx, dtype, cuda, seed=11), C, layout, K, seed=12)
+    gamma, beta = _affine(C, cuda, seed=13)
+    _, y, _ = _run(x, gamma, beta, B, HW, C, ldy, dtype, eps, True)
+    e = worst_group_rel_l2(y, _reference(x, C, gamma, beta, eps, True), C)
+    print(f'GN outlier {layout:6} K={K!s:>3} {"bf16" if dtype == BF else "fp16"} {_label(shape[:6])} '
+          f'[{gn_mode}: {_expected(gn_mode, B, HW, C, ldx, ldy)}] worst group rel-L2 {e:.2e}')
+    assert torch.isfinite(y).all()
     assert e < TOL[dtype]
 
 
