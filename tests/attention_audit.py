@@ -488,99 +488,20 @@ def record(entry, abi, S):
     return {'op': 'fwd', 'abi': a, 'in': x, 'targets': targets, 'pre': pre}
 
 
-def attach_mem(rec, S):
-    """snapshot every storage the launch may write into rec['mem'][...]['before']; -> their live flat views"""
-    flats = {k: S.flat(*k) for k in {t['mem'] for t in rec['targets']}}
-    rec['mem'] = {k: {'before': f.clone()} for k, f in flats.items()}
-    return flats
-
-
 # --------------------------------------------------------------------------------------------------- recorder
 _OPS = ('attention', 'attention_train', 'attention_causal', 'attention_bwd', 'attn_delta', 'heads_transpose')
 
 
-def _sync(tensors):
-    if any(t.is_cuda for t in tensors):
-        torch.cuda.synchronize()
+class Recorder(ga.LaunchRecorder):
+    """audits every attention-family launch made inside it"""
+    OPS = _OPS
+    ENTRY_POINTS = ENTRY_POINTS
 
+    def record(self, entry, args, S):
+        return record(entry, abi_of(entry, args[:len(_ARGS[entry])]), S)
 
-class Recorder:
-    """Context manager: audits every attention-family launch made inside it (eager walks only).  It works on CPU tensors
-    too, with a stand-in library in place of `_lib.lib()`."""
+    def key(self, rec):
+        return attn_path(rec)
 
-    def __init__(self, stats=None, determinism='all'):
-        self.stats = stats if stats is not None else Stats()
-        self.determinism = determinism
-        self._ctx = None
-
-    def __enter__(self):
-        from mos_b200 import _lib, ops
-        self._ops, self._libmod = ops, _lib
-        self._orig_ops = {n: getattr(ops, n) for n in _OPS}
-        self._orig_lib = _lib.lib
-        real = _lib.lib()
-        rec = self
-
-        class Proxy:
-            def __getattr__(self, name):
-                if name in ENTRY_POINTS:
-                    fn = getattr(real, name)
-                    return lambda *args: rec._audit(name, lambda: fn(*args), args)
-                return getattr(real, name)
-
-        proxy = Proxy()
-
-        def wrap(fn):
-            def _audited(*args, **kwargs):
-                assert self._ctx is None
-                self._ctx = (ga._tensors(args, kwargs), ga._site())
-                try:
-                    return fn(*args, **kwargs)
-                finally:
-                    self._ctx = None
-            return _audited
-
-        for n, fn in self._orig_ops.items():
-            setattr(ops, n, wrap(fn))
-        _lib.lib = lambda: proxy
-        return self
-
-    def __exit__(self, *exc):
-        for n, fn in self._orig_ops.items():
-            setattr(self._ops, n, fn)
-        self._libmod.lib = self._orig_lib
-        return False
-
-    def _audit(self, entry, launch, args):
-        assert self._ctx is not None, f'{entry} launched outside the ops.* attention wrappers'
-        tensors, site = self._ctx
-        if any(t.is_cuda for t in tensors):
-            assert not torch.cuda.is_current_stream_capturing(), 'the launch audit needs an eager walk (use_graph=False)'
-        _sync(tensors)
-        S = _Storages(tensors)
-        rec = record(entry, abi_of(entry, args[:len(_ARGS[entry])]), S)
-        key = attn_path(rec)
-        live, rec['in'] = rec['in'], {k: v.clone() for k, v in rec['in'].items()}
-        flats = attach_mem(rec, S)
-        rc = launch()
-        _sync(tensors)
-        if rc != 0:
-            return rc
-        for k, f in flats.items():
-            rec['mem'][k]['after'] = f.clone()
-        res = check_launch(rec)
-        for k, v in rec['in'].items():
-            if not torch.equal(v.reshape(-1).view(_BITS[v.element_size()]),
-                               live[k].reshape(-1).view(_BITS[v.element_size()])):
-                res['errors'].append(f'(d) operand {k} changed by the launch')
-        if self.determinism == 'all' or key not in self.stats.rows:
-            for k, f in flats.items():
-                f.copy_(rec['mem'][k]['before'])
-            assert launch() == 0
-            _sync(tensors)
-            for k, f in flats.items():
-                if not torch.equal(f.view(_BITS[f.element_size()]), rec['mem'][k]['after'].view(_BITS[f.element_size()])):
-                    res['errors'].append('(e) a second launch from the same bytes is not bit-identical')
-        self.stats.add(key, site, res)
-        self.last = rec
-        return rc
+    def check(self, rec):
+        return check_launch(rec)

@@ -14,8 +14,10 @@ def sd15_pair():
     return unet, {k: v.clone() for k, v in unet.state_dict().items()}
 
 
-def _run(audit, fn):
-    with audit():
+def _run(audit, fn, register=()):
+    """register: tensors that device pointer tables of the call may point into"""
+    with audit() as rec:
+        rec.register(*register)
         out = fn()
         torch.cuda.synchronize()
     return out
@@ -52,9 +54,11 @@ def sample_96x192_whole_block(sd15, audit):
     _run(audit, lambda: eng.forward(lat.cuda(), torch.tensor([501.0, 501.0]).cuda(), ehs_to_layer_major(ehs.cuda())))
 
 
-def train_sd15_channels_whole_block(audit, attn_reg_weight=None):
+def train_sd15_channels_whole_block(audit, attn_reg_weight=None, optimizer_step=False):
     """bf16 TrainEngine.forward_backward at the SD1.5 channels, one layer per block, 16 x 16, B = 2, whole-block LoRA;
-    with attn_reg_weight the regulariser runs (pcols / pos / gcols) on a box mask with concept tokens at 4, 5 / 6, 7"""
+    with attn_reg_weight the regulariser runs (pcols / pos / gcols) on a box mask with concept tokens at 4, 5 / 6, 7;
+    with optimizer_step the AdamW step and the LoRA re-pack (its table points into the flat state and the GEMM
+    operands, registered with the audit) follow"""
     from mos_b200.engine import ehs_to_layer_major
     from mos_b200.train_engine import TrainEngine
     from oracle import inject
@@ -77,6 +81,37 @@ def train_sd15_channels_whole_block(audit, attn_reg_weight=None):
         pos = [[4, 5], [6, 7]]
     _run(audit, lambda: eng.forward_backward(x0.cuda(), noise.cuda(), torch.tensor([77, 640]).cuda(),
                                              ehs_to_layer_major(ehs.cuda(), n_x), masks.cuda(), token_pos=pos))
+    if optimizer_step:
+        packed = [e[k] for e in eng.w.values() if isinstance(e, dict) for k in ('lora_down', 'lora_up')
+                  if isinstance(e.get(k), torch.Tensor)]
+        _run(audit, eng.optimizer_step, register=[eng.state.params, *eng._lora_keep, *packed])
+
+
+def vae_512(audit):
+    """VAEEngine at 512 x 512 with the SD1.5 VAE widths: encode with a noise draw, then decode"""
+    from mos_b200.vae_engine import VAEEngine
+    from oracle import vae as ov
+    ref = ov.build_vae(0, None)
+    full = dict(ov.SD15_VAE)
+    sd = {k: v.detach().clone() for k, v in ref.state_dict().items()}
+    eng = VAEEngine(sd, 1, 512, 512, block_out=full['block_out_channels'], layers=full['layers_per_block'])
+    g = torch.Generator().manual_seed(1)
+    img = torch.rand(1, 3, 512, 512, generator=g) * 2 - 1
+    noise, z = torch.randn(1, 4, 64, 64, generator=g), torch.randn(1, 4, 64, 64, generator=g)
+    _run(audit, lambda: eng.encode(img.cuda(), noise=noise.cuda()))
+    _run(audit, lambda: eng.decode(z.cuda()))
+
+
+def sampling_loop(audit, tmp_dir):
+    """EDLoRAPipeline on a synthetic pretrained directory: 64 x 64, 3 DPM-Solver++ steps with CFG, latent output, eager
+    UNet (the CFG / DPM update with the next timestep written for the following UNet call)"""
+    from mixofshow.pipelines.pipeline_edlora import EDLoRAPipeline
+    from synth import make_pretrained_dir
+    pipe = EDLoRAPipeline.from_pretrained(make_pretrained_dir(str(tmp_dir)))
+    pipe.set_new_concept_cfg({})                     # no concept tokens: every layer reads the plain prompt
+    pipe.unet.use_graph = False
+    _run(audit, lambda: pipe('photo of a cat', negative_prompt='blurry', height=64, width=64, num_inference_steps=3,
+                             guidance_scale=7.5, output_type='latent'))
 
 
 def clip_text_and_train(audit, device):

@@ -393,27 +393,34 @@ def abi_of(args):
 
 
 class _Storages:
-    """the storages of a call's tensor arguments; maps a device pointer to (storage, byte offset)"""
+    """the storages of a call's tensor arguments; maps a device pointer to (storage, byte offset).  `extra`: storages
+    that only pointers read from a device table may resolve into (find(..., table=True))"""
 
-    def __init__(self, tensors):
-        self.st = {}
+    def __init__(self, tensors, extra=()):
+        self.st, self.extra = {}, {}
         for t in tensors:
             s = t.untyped_storage()
             self.st[s.data_ptr()] = (s, t.device)
+        for t in extra:
+            s = t.untyped_storage()
+            self.extra.setdefault(s.data_ptr(), (s, t.device))
 
-    def find(self, p, what):
-        for base, (s, dev) in self.st.items():
-            if base <= p < base + s.nbytes():
-                return base, p - base
-        raise AssertionError(f'{what}: pointer {p:#x} lies in no tensor argument of the call')
+    def find(self, p, what, table=False):
+        for pool in (self.st, self.extra) if table else (self.st,):
+            for base, (s, dev) in pool.items():
+                if base <= p < base + s.nbytes():
+                    return base, p - base
+        raise AssertionError(f'{what}: pointer {p:#x} lies in no ' +
+                             ('tensor argument of the call or registered tensor' if table
+                              else 'tensor argument of the call'))
 
     def flat(self, base, dtype):
-        s, dev = self.st[base]
+        s, dev = self.st[base] if base in self.st else self.extra[base]
         es = torch.empty(0, dtype=dtype).element_size()
         return torch.empty(0, dtype=dtype, device=dev).set_(s, 0, (s.nbytes() // es,), (1,))
 
-    def window(self, p, what, dtype, size, stride):
-        base, off = self.find(p, what)
+    def window(self, p, what, dtype, size, stride, table=False):
+        base, off = self.find(p, what, table)
         es = torch.empty(0, dtype=dtype).element_size()
         assert off % es == 0, f'{what}: pointer not aligned to its element size'
         try:
@@ -425,19 +432,23 @@ class _Storages:
 def _site():
     for fr in reversed(traceback.extract_stack()[:-1]):
         f = fr.filename.replace('\\', '/')
-        if f.endswith(('/ops.py', '/gemm_audit.py', '/attention_audit.py')) or fr.name in ('gemm', '_audited'):
+        if f.endswith(('/ops.py', '/gemm_audit.py', '/attention_audit.py', '/norm_audit.py')) or \
+                fr.name in ('gemm', '_audited', '_registering'):
             continue
         return f"{f.rsplit('/', 1)[-1]}:{fr.lineno}"
     return '?'
 
 
 def _tensors(args, kwargs):
+    """the tensors among a call's arguments: lists and tuples are flattened, a heads dict contributes its seg_ptr"""
     out = []
     for v in list(args) + list(kwargs.values()):
         if isinstance(v, torch.Tensor):
             out.append(v)
+        elif isinstance(v, (list, tuple)):
+            out += _tensors(v, {})
         elif isinstance(v, dict):
-            out += [t for t in v.get('seg_ptr', ()) if isinstance(t, torch.Tensor)]
+            out += _tensors(v.get('seg_ptr', ()), {})
     return out
 
 
@@ -554,90 +565,148 @@ class Stats:
         return '\n'.join(lines)
 
 
-class Recorder:
-    """Context manager: audits every ops.gemm / ops.splitk_finalize launch made inside it (eager walks only).
+class LaunchRecorder:
+    """Context manager shared by the launch audits: wraps the `ops.*` functions named in OPS, proxies `_lib.lib()` so that
+    every call of an entry point in ENTRY_POINTS made inside one of them is audited, and restores both on exit (eager
+    walks only; it works on CPU tensors too, with a stand-in library in place of `_lib.lib()`).
+
+    A subclass supplies `record(entry, args, S)` (the launch record, built from the ABI arguments and the storages S of
+    the call's tensor arguments), `key(rec)` and `check(rec)`.  Each launch is checked by `check` ((p), (a)-(c)); the
+    recorder adds (d) the operand windows rec['in'] are unchanged, except the names in rec['inplace'], and (e) one more
+    launch from the same bytes is bit-identical.  The tensor arguments of the ops in REGISTER_OPS are kept as storages
+    that device pointer tables may point into (S.find resolves them like tensor arguments).
     determinism: 'all' relaunches every launch once more, 'first' only the first launch of each path key."""
+    OPS = ()
+    ENTRY_POINTS = ()
+    REGISTER_OPS = ()
 
     def __init__(self, stats=None, determinism='all'):
         self.stats = stats if stats is not None else Stats()
         self.determinism = determinism
         self._ctx = None
+        self.registered = []
+        self.last = None
+
+    def register(self, *tensors):
+        """storages a pointer table of a later launch may point into"""
+        self.registered += _tensors(tensors, {})
+
+    def record(self, entry, args, S):
+        raise NotImplementedError
+
+    def key(self, rec):
+        raise NotImplementedError
+
+    def check(self, rec):
+        raise NotImplementedError
 
     def __enter__(self):
         from mos_b200 import _lib, ops
         self._ops, self._libmod = ops, _lib
-        self._orig = (ops.gemm, ops.splitk_finalize, _lib.lib)
+        self._orig_ops = {n: getattr(ops, n) for n in self.OPS + self.REGISTER_OPS}
+        self._orig_lib = _lib.lib
         real = _lib.lib()
         rec = self
 
         class Proxy:
             def __getattr__(self, name):
-                return getattr(real, name)
-
-            def mos_gemm_bf16(self, argref, stream):
-                return rec._audit(lambda: real.mos_gemm_bf16(argref, stream), 'gemm', argref._obj)
-
-            def mos_splitk_finalize(self, *args):
-                return rec._audit(lambda: real.mos_splitk_finalize(*args), 'finalize', args)
+                fn = getattr(real, name)
+                if name in rec.ENTRY_POINTS:
+                    return lambda *args: rec._audit(name, lambda: fn(*args), args)
+                return fn
 
         proxy = Proxy()
 
         def wrap(fn):
             def _audited(*args, **kwargs):
                 assert self._ctx is None
-                self._ctx = (_tensors(args, kwargs), _site())
+                self._ctx = (_tensors(args, kwargs), _site(), (args, kwargs))
                 try:
                     return fn(*args, **kwargs)
                 finally:
                     self._ctx = None
             return _audited
 
-        ops.gemm, ops.splitk_finalize = wrap(self._orig[0]), wrap(self._orig[1])
+        def registering(fn):
+            def _registering(*args, **kwargs):
+                self.register(*args, *kwargs.values())
+                return fn(*args, **kwargs)
+            return _registering
+
+        for n, fn in self._orig_ops.items():
+            setattr(ops, n, wrap(fn) if n in self.OPS else registering(fn))
         _lib.lib = lambda: proxy
         return self
 
     def __exit__(self, *exc):
-        self._ops.gemm, self._ops.splitk_finalize, self._libmod.lib = self._orig
+        for n, fn in self._orig_ops.items():
+            setattr(self._ops, n, fn)
+        self._libmod.lib = self._orig_lib
+        self.registered = []
         return False
 
-    def _audit(self, launch, op, args):
-        assert self._ctx is not None, f'{op} launched outside ops.gemm / ops.splitk_finalize'
-        assert not torch.cuda.is_current_stream_capturing(), 'the launch audit needs an eager walk (use_graph=False)'
-        tensors, site = self._ctx
-        torch.cuda.synchronize()
-        S = _Storages(tensors)
-        if op == 'gemm':
-            rec = gemm_record(abi_of(args), S)
-        else:
-            vals = [getattr(v, 'value', v) for v in args[:13]]
-            rec = finalize_record([0 if v is None else int(v) for v in vals], S)
-        key = gemm_path(rec)
+    def _audit(self, entry, launch, args):
+        assert self._ctx is not None, f'{entry} launched outside the audited ops.* wrappers'
+        tensors, site = self._ctx[:2]
+        cuda = any(t.is_cuda for t in tensors)
+        if cuda:
+            assert not torch.cuda.is_current_stream_capturing(), 'the launch audit needs an eager walk (use_graph=False)'
+            torch.cuda.synchronize()
+        S = _Storages(tensors, self.registered)
+        rec = self.record(entry, args, S)
+        key = self.key(rec)
         live, rec['in'] = rec['in'], {k: v.clone() for k, v in rec['in'].items()}   # the reference reads the snapshot
         flats = attach_mem(rec, S)
-        zero = {k: S.flat(k, torch.int32) for k in rec['zero']}
+        zero = {k: S.flat(k, torch.int32) for k in rec.get('zero', ())}
         for k, z in zero.items():
             assert (z == 0).all(), 'split-K tile counters must be zero before the launch'
-        rc = launch()
-        torch.cuda.synchronize()
+
+        def run():
+            rc = launch()
+            if cuda:
+                torch.cuda.synchronize()
+            return rc
+        rc = run()
         if rc != 0:
             return rc
         for k, f in flats.items():
             rec['mem'][k]['after'] = f.clone()
         rec['zero_after'] = {k: z.clone() for k, z in zero.items()}
-        res = check_launch(rec)
-        alias = op == 'gemm' and rec['abi']['residual'] == rec['abi']['out']
+        res = self.check(rec)
         for k, v in rec['in'].items():
-            if k == 'residual' and alias:
-                continue                                 # a residual that aliases `out` is read and then overwritten
-            if not torch.equal(v.view(_BITS[v.element_size()]), live[k].view(_BITS[v.element_size()])):
+            if k in rec.get('inplace', ()):
+                continue                                 # read and then overwritten by the launch
+            if not torch.equal(v.reshape(-1).view(_BITS[v.element_size()]),
+                               live[k].reshape(-1).view(_BITS[v.element_size()])):
                 res['errors'].append(f'(d) operand {k} changed by the launch')
         if self.determinism == 'all' or key not in self.stats.rows:
             for k, f in flats.items():
                 f.copy_(rec['mem'][k]['before'])
-            assert launch() == 0
-            torch.cuda.synchronize()
+            assert run() == 0
             for k, f in flats.items():
                 if not torch.equal(f.view(_BITS[f.element_size()]), rec['mem'][k]['after'].view(_BITS[f.element_size()])):
                     res['errors'].append('(e) a second launch from the same bytes is not bit-identical')
         self.stats.add(key, site, res)
+        self.last = rec
         return rc
+
+
+class Recorder(LaunchRecorder):
+    """audits every ops.gemm / ops.splitk_finalize launch made inside it"""
+    OPS = ('gemm', 'splitk_finalize')
+    ENTRY_POINTS = ('mos_gemm_bf16', 'mos_splitk_finalize')
+
+    def record(self, entry, args, S):
+        if entry == 'mos_gemm_bf16':
+            rec = gemm_record(abi_of(args[0]._obj), S)
+            if rec['abi']['residual'] and rec['abi']['residual'] == rec['abi']['out']:
+                rec['inplace'] = ('residual',)           # a residual that aliases `out` is read and then overwritten
+            return rec
+        vals = [getattr(v, 'value', v) for v in args[:13]]
+        return finalize_record([0 if v is None else int(v) for v in vals], S)
+
+    def key(self, rec):
+        return gemm_path(rec)
+
+    def check(self, rec):
+        return check_launch(rec)

@@ -137,17 +137,7 @@ def test_clip_text_and_train(cuda):
 
 
 def test_vae_512(cuda):
-    from mos_b200.vae_engine import VAEEngine
-    from oracle import vae as ov
-    ref = ov.build_vae(0, None)
-    full = dict(ov.SD15_VAE)
-    sd = {k: v.detach().clone() for k, v in ref.state_dict().items()}
-    eng = VAEEngine(sd, 1, 512, 512, block_out=full['block_out_channels'], layers=full['layers_per_block'])
-    g = torch.Generator().manual_seed(1)
-    img = torch.rand(1, 3, 512, 512, generator=g) * 2 - 1
-    noise, z = torch.randn(1, 4, 64, 64, generator=g), torch.randn(1, 4, 64, 64, generator=g)
-    _audited(lambda: eng.encode(img.cuda(), noise=noise.cuda()))
-    _audited(lambda: eng.decode(z.cuda()))
+    walks.vae_512(lambda: ga.Recorder(STATS))
 
 
 def test_fusion_gram_whole_block(cuda):
