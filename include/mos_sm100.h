@@ -195,6 +195,20 @@ int mos_vae_moments(const void* h, int64_t ldh, int32_t B, int64_t HW, int32_t L
                     float* mean, float* logvar, const float* noise, float scaling, float* latents, int32_t act_dtype,
                     void* stream);
 
+/* ---- T2I-Adapter (diffusers T2IAdapter, adapter_type 'full_adapter': pipeline_regionally_t2iadapter.py:474-482, once per
+ * image).  Its 3x3 / 1x1 convolutions and the resnet adds are mos_gemm_bf16 launches; these supply the layout and
+ * elementwise steps between them.  16-bit tensors are NHWC rows of type act_dtype. */
+/* PixelUnshuffle(8): fp32 NCHW [B, Cin, H, W] -> [B*(H/8)*(W/8), ldy] with column c*64 + i*8 + j = x[b, c, 8h+i, 8w+j]
+ * (columns 64 Cin .. ldy-1 untouched); H, W multiples of 8. */
+int mos_pixel_unshuffle(const float* x, int32_t B, int32_t Cin, int32_t H, int32_t W, void* y, int64_t ldy,
+                        int32_t act_dtype, void* stream);
+/* x[m, :C] <- (x < 0 ? 0 : x) in place (ReLU; NaN passes through). */
+int mos_relu_rows(void* x, int64_t ld, int64_t M, int32_t C, int32_t act_dtype, void* stream);
+/* AvgPool2d(2, 2): [B, H, W, C] at pixel pitch ldx -> [B, H/2, W/2, C] at pitch ldy; fp32 sum of the 4 taps times 0.25, one
+ * rounding; H, W even. */
+int mos_avgpool2x(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, void* y, int64_t ldy,
+                  int32_t act_dtype, void* stream);
+
 /* One fused kernel for mixofshow/pipelines/pipeline_edlora.py:273-290: classifier-free-guidance combine,
  * DPM-Solver++(2M) data-prediction update and re-duplication of the latents for the next UNet call.
  * noise_pred fp32 [2n] (uncond | cond) when cfg else [n]; coefficients from the host-side schedule.

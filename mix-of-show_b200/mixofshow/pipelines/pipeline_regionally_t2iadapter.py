@@ -4,8 +4,9 @@
 The region-masked cross-attention (reference :32-86) runs as: one flash cross-attention per region with the region's
 own K/V (wgmma), then `mos_region_combine` (global outside the boxes, mean of covering regions inside).  Box indices
 are computed on the host in Python float64 exactly as the reference does (`math.ceil` / `math.floor`), so they are
-bit-exact.  The T2I-Adapter networks themselves are out of scope (SURVEY.md §2.1 row 6): pass their four feature
-maps as `adapter_state` (or torch adapter modules as `keypose_adapter` / `sketch_adapter` attributes).
+bit-exact.  Condition images (`keypose_adapter_input` / `sketch_adapter_input`) are preprocessed as diffusers does and
+run once per call through `pipe.keypose_adapter` / `pipe.sketch_adapter`, normally `mixofshow.models.adapter_b200.T2IAdapter`
+(the adapter network on the GPU); precomputed feature maps can still be passed as `*_adapter_state`.
 """
 import ast
 import math
@@ -87,6 +88,30 @@ def _spatial_weight(feat, base_weight, region_weight_str, height, width):
     return wmap * feat
 
 
+def preprocess_adapter_image(image, height, width):
+    """Condition image(s) -> fp32 NCHW batch in [0, 1], as diffusers' `_preprocess_adapter_image` (called at reference
+    :413-423): a PIL image or a list of them is resized with LANCZOS to (width, height), a 2-D (grayscale) array gets a
+    channel axis, values are divided by 255 and moved to NCHW; tensors pass through (a list of 3-D tensors is stacked,
+    of 4-D tensors concatenated)."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(image, torch.Tensor):
+        return image
+    if isinstance(image, Image.Image):
+        image = [image]
+    if isinstance(image[0], Image.Image):
+        arrs = [np.array(im.resize((width, height), resample=Image.LANCZOS)) for im in image]
+        arrs = [a[None, :, :, None] if a.ndim == 2 else a[None] for a in arrs]
+        batch = np.concatenate(arrs, 0).astype(np.float32) / 255.0
+        return torch.from_numpy(batch.transpose(0, 3, 1, 2).copy())
+    if isinstance(image[0], torch.Tensor):
+        if image[0].ndim == 3:
+            return torch.stack(image, 0)
+        if image[0].ndim == 4:
+            return torch.cat(image, 0)
+    raise ValueError(f'unsupported adapter condition input {type(image[0]).__name__}')
+
+
 class RegionallyT2IAdapterPipeline:
     def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None, safety_checker=None,
                  feature_extractor=None, requires_safety_checker: bool = False):
@@ -106,6 +131,15 @@ class RegionallyT2IAdapterPipeline:
 
     def set_new_concept_cfg(self, new_concept_cfg=None):
         self.new_concept_cfg = new_concept_cfg
+
+    @staticmethod
+    def _run_adapter(adapter, image, height, width, device):
+        """reference :413-423 + :474-482: preprocess the condition, move it to the device in the adapter's dtype, run it"""
+        if adapter is None:
+            raise ValueError('a condition image was given but no adapter is attached (set pipe.keypose_adapter / '
+                             'pipe.sketch_adapter, e.g. mixofshow.models.adapter_b200.T2IAdapter.from_pretrained(dir))')
+        x = preprocess_adapter_image(image, height, width)
+        return adapter(x.to(device, getattr(adapter, 'dtype', torch.float32)))
 
     def _embed(self, prompts, device):
         ids = self.tokenizer(prompts, padding='max_length', max_length=self.tokenizer.model_max_length,
@@ -152,7 +186,8 @@ class RegionallyT2IAdapterPipeline:
                  return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None,
                  region_list=None, keypose_adapter_state=None, sketch_adapter_state=None):
         """Extra (GPU path) arguments: `region_list` = [(region_embeds [2,16,77,768], box fractions)] and
-        `*_adapter_state` = precomputed T2I-Adapter feature maps (4 NCHW tensors), for use without CLIP / adapters."""
+        `*_adapter_state` = precomputed T2I-Adapter feature maps (4 NCHW tensors), for use without CLIP / adapters; a
+        state takes the place of the adapter run on the matching `*_adapter_input`."""
         device = self.device
         do_cfg = guidance_scale > 1.0
         assert self.new_concept_cfg is not None
@@ -170,9 +205,9 @@ class RegionallyT2IAdapterPipeline:
         latents = (latents.to(device, torch.float32) * self.scheduler.init_noise_sigma).contiguous()
 
         if keypose_adapter_state is None and keypose_adapter_input is not None:
-            keypose_adapter_state = self.keypose_adapter(keypose_adapter_input)
+            keypose_adapter_state = self._run_adapter(self.keypose_adapter, keypose_adapter_input, height, width, device)
         if sketch_adapter_state is None and sketch_adapter_input is not None:
-            sketch_adapter_state = self.sketch_adapter(sketch_adapter_input)
+            sketch_adapter_state = self._run_adapter(self.sketch_adapter, sketch_adapter_input, height, width, device)
         adapter_state = None
         if keypose_adapter_state is not None or sketch_adapter_state is not None:
             n = len(keypose_adapter_state) if keypose_adapter_state is not None else len(sketch_adapter_state)

@@ -5,6 +5,8 @@
         <dir>/unet/config.json + diffusion_pytorch_model.safetensors (or .bin)
         <dir>/text_encoder/config.json + model.safetensors (or pytorch_model.bin)
   * `<dir>/new_concept_cfg.json` (`gradient_fusion.py:812-813`).
+  * a diffusers T2I-Adapter directory (`config.json` + `diffusion_pytorch_model.safetensors` or `.bin`), the layout of the
+    adapters `regionally_controlable_sampling.py:62-63` loads.
 
 `load_unet` / `load_text_encoder` build this repo's GPU containers from such a directory; `save_combined_model` writes
 one.  diffusers itself is not a dependency: the UNet `config.json` keys are the SD1.5 ones (diffusers 0.19.3), and any
@@ -170,6 +172,42 @@ def save_vae(vae, model_dir, subfolder='vae'):
     with open(os.path.join(folder, 'config.json'), 'w') as f:
         json.dump(cfg, f, indent=2, sort_keys=True)
     _write_weights(folder, VAE_WEIGHTS[0], vae.state_dict())
+
+
+ADAPTER_WEIGHTS = ('diffusion_pytorch_model.safetensors', 'diffusion_pytorch_model.bin')
+
+
+def load_t2i_adapter(model_dir, subfolder=None, device='cuda'):
+    """diffusers-layout T2I-Adapter directory (config.json + weights) -> mixofshow.models.adapter_b200.T2IAdapter.  Hub ids
+    (e.g. 'TencentARC/t2iadapter_openpose_sd14v1') are not fetched: download the adapter and pass its directory."""
+    from mixofshow.models.adapter_b200 import T2IAdapter
+    folder = os.path.join(model_dir, subfolder) if subfolder else model_dir
+    if not os.path.isdir(folder):
+        raise ValueError(f'T2I-Adapter: {folder!r} is not a local directory; hub ids are not downloaded, pass the '
+                         'directory that holds config.json and diffusion_pytorch_model.safetensors (or .bin)')
+    with open(os.path.join(folder, 'config.json')) as f:
+        cfg = json.load(f)
+    return T2IAdapter(_read_weights(folder, ADAPTER_WEIGHTS), in_channels=cfg.get('in_channels', 3),
+                      channels=tuple(cfg.get('channels', (320, 640, 1280, 1280))),
+                      num_res_blocks=cfg.get('num_res_blocks', 2), downscale_factor=cfg.get('downscale_factor', 8),
+                      adapter_type=cfg.get('adapter_type', 'full_adapter'), device=device)
+
+
+def save_t2i_adapter(adapter, model_dir, subfolder=None, safe_serialization=True):
+    """write `adapter` (anything with .config and .state_dict()) in the diffusers layout: safetensors, or the .bin pickle"""
+    folder = os.path.join(model_dir, subfolder) if subfolder else model_dir
+    c = adapter.config
+    cfg = {'_class_name': 'T2IAdapter', '_diffusers_version': '0.19.3', 'adapter_type': c.adapter_type,
+           'channels': list(c.channels), 'downscale_factor': c.downscale_factor, 'in_channels': c.in_channels,
+           'num_res_blocks': c.num_res_blocks}
+    os.makedirs(folder, exist_ok=True)
+    with open(os.path.join(folder, 'config.json'), 'w') as f:
+        json.dump(cfg, f, indent=2, sort_keys=True)
+    if safe_serialization:
+        _write_weights(folder, ADAPTER_WEIGHTS[0], adapter.state_dict())
+    else:
+        torch.save({k: v.detach().to('cpu').contiguous() for k, v in adapter.state_dict().items()},
+                   os.path.join(folder, ADAPTER_WEIGHTS[1]))
 
 
 def save_combined_model(model_dir, unet, text_encoder, new_concept_cfg, tokenizer=None):

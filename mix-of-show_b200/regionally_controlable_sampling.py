@@ -2,10 +2,10 @@
 parsing, model loading from a fused `combined_model_*` directory, and the sampling call.  Host logic only; the UNet loop runs
 on `RegionallyT2IAdapterPipeline` (mixofshow/pipelines/pipeline_regionally_t2iadapter.py).
 
-Out of scope here (SURVEY.md §2.1 row 6 / §8f): the T2I-Adapter networks and the VAE.  Conditions are therefore passed as
+Conditions are condition images (`--keypose_condition` / `--sketch_condition`, as in the reference) run through T2I-Adapters
+loaded from LOCAL directories (`--keypose_adapter` / `--sketch_adapter`: the reference downloads them from the hub), or
 pre-computed adapter feature maps (`--keypose_adapter_state` / `--sketch_adapter_state file.pt`: the 4 maps a T2IAdapter
-returns) or skipped, and the result is
-written as latents unless a VAE object is supplied."""
+returns).  Out of scope here (SURVEY.md §8f): the VAE, so the result is written as latents."""
 import argparse
 import ast
 import json
@@ -78,11 +78,44 @@ def parse_args(argv=None):
     parser.add_argument('--seed', default=16141, type=int)
     parser.add_argument('--suffix', default='', type=str)
     parser.add_argument('--num_inference_steps', default=50, type=int)       # the reference samples with 50 steps (:38)
+    parser.add_argument('--sketch_condition', default=None, type=str, help='sketch condition image (opened as L)')
+    parser.add_argument('--keypose_condition', default=None, type=str, help='key-pose condition image (opened as RGB)')
+    parser.add_argument('--sketch_adapter', default=None, type=str, help='local T2I-Adapter directory for --sketch_condition')
+    parser.add_argument('--keypose_adapter', default=None, type=str,
+                        help='local T2I-Adapter directory for --keypose_condition')
     return parser.parse_args(argv)
+
+
+CONDITION_ARGS = ('sketch_condition', 'keypose_condition', 'sketch_adapter', 'keypose_adapter')
+_MODES = {'sketch': 'L', 'keypose': 'RGB'}           # reference :118-130
+
+
+def load_conditions(args):
+    """reference :118-135: open the condition images (sketch as 'L', key pose as 'RGB'); when any is given, height and width
+    become its size (two conditions must agree) and are written back to `args`.  -> {kind: PIL image}.  A condition needs
+    its adapter directory (the reference's hub downloads are not made here) and excludes a precomputed state."""
+    from PIL import Image
+    conds = {}
+    for kind, mode in _MODES.items():
+        path = getattr(args, f'{kind}_condition')
+        if path is None:
+            continue
+        if getattr(args, f'{kind}_adapter') is None:
+            raise ValueError(f'--{kind}_condition needs --{kind}_adapter (a local T2I-Adapter directory)')
+        if getattr(args, f'{kind}_adapter_state') is not None:
+            raise ValueError(f'--{kind}_condition and --{kind}_adapter_state both give the {kind} adapter features')
+        conds[kind] = Image.open(path).convert(mode)
+    sizes = {im.size for im in conds.values()}
+    if len(sizes) > 1:
+        raise ValueError(f'conditions should be same size, got (width, height) {sorted(sizes)}')
+    if sizes:
+        args.width, args.height = sizes.pop()
+    return conds
 
 
 def main(argv=None):
     args = parse_args(argv)
+    conds = load_conditions(args)
     device = torch.device('cuda')
     pipe = build_model(args.pretrained_model, device)
     kwargs = {'height': args.height, 'width': args.width, 'output_type': 'latent'}
@@ -90,6 +123,10 @@ def main(argv=None):
         path = getattr(args, f'{kind}_adapter_state')
         if path is not None:
             kwargs[f'{kind}_adapter_state'] = torch.load(path)
+        if kind in conds:
+            from mixofshow.models.adapter_b200 import T2IAdapter
+            setattr(pipe, f'{kind}_adapter', T2IAdapter.from_pretrained(getattr(args, f'{kind}_adapter'), device=device))
+            kwargs[f'{kind}_adapter_input'] = [conds[kind]]
         kwargs[f'{kind}_adaptor_weight'] = getattr(args, f'{kind}_adaptor_weight')
         kwargs[f'region_{kind}_adaptor_weight'] = getattr(args, f'region_{kind}_adaptor_weight')
     input_prompt = [prepare_text(args.prompt, args.prompt_rewrite, args.height, args.width)]
@@ -99,9 +136,11 @@ def main(argv=None):
     if args.save_dir is not None:
         os.makedirs(args.save_dir, exist_ok=True)
         out = os.path.join(args.save_dir, f'latents---{args.seed}{"---" + args.suffix if args.suffix else ""}.pt')
-        torch.save({'latents': latents.cpu(), 'config': vars(args)}, out)
+        # condition options that were not given are left out, so an unconditioned run records what it always did
+        config = {k: v for k, v in vars(args).items() if not (k in CONDITION_ARGS and v is None)}
+        torch.save({'latents': latents.cpu(), 'config': config}, out)
         with open(os.path.join(args.save_dir, 'config.json'), 'w') as f:
-            json.dump(vars(args), f)
+            json.dump(config, f)
         print(f'save to: {out}')
     return latents
 
