@@ -192,6 +192,9 @@ dgemm_mixed_kernel(const float* __restrict__ A, const double* __restrict__ B, do
 }
 
 // ------------------------------------------------------------------ deterministic block reductions
+// max that propagates NaN (fmaxf drops it): a NaN gradient must not pass the solver's convergence tests, as with torch's
+// abs().max()
+__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
 __device__ __forceinline__ float block_sum(float v, float* sh) {
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
@@ -208,14 +211,14 @@ __device__ __forceinline__ float block_sum(float v, float* sh) {
 }
 __device__ __forceinline__ float block_max(float v, float* sh) {
 #pragma unroll
-  for (int d = 16; d > 0; d >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, d));
+  for (int d = 16; d > 0; d >>= 1) v = nan_max(v, __shfl_xor_sync(0xffffffffu, v, d));
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
   __syncthreads();
   float r = 0.f;
   if (threadIdx.x < 32) {
     r = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.f;
 #pragma unroll
-    for (int d = 16; d > 0; d >>= 1) r = fmaxf(r, __shfl_xor_sync(0xffffffffu, r, d));
+    for (int d = 16; d > 0; d >>= 1) r = nan_max(r, __shfl_xor_sync(0xffffffffu, r, d));
   }
   __syncthreads();
   return r;
@@ -262,7 +265,7 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int nb
                                        float* __restrict__ out) {
   __shared__ float sh[32];
   float v = 0.f;
-  for (int i = threadIdx.x; i < nb; i += blockDim.x) v = is_max ? fmaxf(v, partial[i]) : v + partial[i];
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) v = is_max ? nan_max(v, partial[i]) : v + partial[i];
   const float t = is_max ? block_max(v, sh) : block_sum(v, sh);
   if (threadIdx.x == 0) out[0] = is_max ? t : scale * t + add;
 }
@@ -287,7 +290,7 @@ __global__ void vec_absmax_kernel(const float* __restrict__ a, long long n, floa
   __shared__ float sh[32];
   float acc = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    acc = fmaxf(acc, fabsf(a[i] * scale));
+    acc = nan_max(acc, fabsf(a[i] * scale));
   const float t = block_max(acc, sh);
   if (threadIdx.x == 0) partial[blockIdx.x] = t;
 }
@@ -445,17 +448,27 @@ extern "C" int mos_dgemm_mixed(const float* A, const double* B, double* C, int32
                                void* stream) {
   MOS_CHECK_ARG(A && B && C && M > 0 && N > 0 && K > 0, "mos_dgemm_mixed: bad arguments");
   constexpr int DK = 32;
-  static int tile_env = -1;
   auto smem = [](int tm, int tn) { return sizeof(double) * 2 * DK * ((tm + 2) + (tn + 2)); };
-  if (tile_env < 0) {
+  // one-time set-up, run once even when several host threads (mos_lbfgs_solve_batch) make their first call together:
+  // a function-local static is initialised exactly once, and the other callers wait for it.  A failed
+  // cudaFuncSetAttribute is kept with it: every later call then returns that error instead of retrying the set-up
+  struct Setup {
+    int tile;
+    cudaError_t err;
+  };
+  static const Setup setup = [&] {
     const char* e = getenv("MOS_DGEMM_TILE");     // 0 = heuristic, 1 = 32 x 64, 2 = 64 x 64, 3 = 64 x 128 (benchmarking)
-    const int v = e ? atoi(e) : 0;
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(dgemm_mixed_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(32, 64)));
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(dgemm_mixed_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(64, 64)));
-    MOS_CHECK_CUDA(cudaFuncSetAttribute(dgemm_mixed_kernel<64, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(64, 128)));
-    tile_env = v;
-  }
-  int tile = tile_env;
+    Setup s{e ? atoi(e) : 0, cudaSuccess};
+    cudaError_t r[3] = {
+        cudaFuncSetAttribute(dgemm_mixed_kernel<32, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(32, 64)),
+        cudaFuncSetAttribute(dgemm_mixed_kernel<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(64, 64)),
+        cudaFuncSetAttribute(dgemm_mixed_kernel<64, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(64, 128))};
+    for (cudaError_t x : r)
+      if (s.err == cudaSuccess) s.err = x;
+    return s;
+  }();
+  MOS_CHECK_CUDA(setup.err);
+  int tile = setup.tile;
   if (tile == 0) tile = 2;   // 64 x 64 by default
   if (tile == 1) {
     dim3 grid((unsigned)ceil_div(N, 64), (unsigned)ceil_div(M, 32));

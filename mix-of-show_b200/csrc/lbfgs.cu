@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <thread>
 #include <vector>
 
@@ -165,7 +166,9 @@ struct Solver {
     loss = h_d[0];
     gtd = dvec != nullptr ? (double)h_f[0] : 0.0;
     ++evals;
-    if (loss < best_loss) {                       // the reference keeps the best iterate of all evaluations (:72-74)
+    // the reference keeps the best iterate of all evaluations (:72-74); a non-finite loss never qualifies, so a solve whose
+    // G or R holds NaN / Inf ends with best_loss = INFINITY and P.best_D unwritten (solve_one then fails)
+    if (std::isfinite(loss) && loss < best_loss) {
       best_loss = loss;
       copy(P.best_D, pt);
     }
@@ -357,7 +360,13 @@ int solve_one(const mos_lbfgs_problem& p, void* workspace, cudaStream_t st) {
   cudaFreeHost(pinned);
   if (p.best_loss != nullptr) *p.best_loss = s.best_loss;
   if (p.n_evals != nullptr) *p.n_evals = s.evals;
+  if (s.rc == MOS_OK && !std::isfinite(s.best_loss)) return MOS_EINVAL;   // no finite evaluation: best_D is unwritten
   return s.rc;
+}
+
+const char* solve_failure(int rc) {
+  return rc == MOS_EINVAL ? "no closure evaluation gave a finite loss (G or R holds NaN or Inf); best_D left unwritten"
+                          : "CUDA error";
 }
 
 bool valid(const mos_lbfgs_problem& p) {
@@ -372,7 +381,9 @@ extern "C" int64_t mos_lbfgs_workspace_bytes(int32_t out_f, int32_t in_f, int32_
 
 extern "C" int mos_lbfgs_solve(const mos_lbfgs_problem* p, void* workspace, void* stream) {
   MOS_CHECK_ARG(p != nullptr && workspace != nullptr && valid(*p), "mos_lbfgs_solve: bad arguments");
-  return solve_one(*p, workspace, reinterpret_cast<cudaStream_t>(stream));
+  const int rc = solve_one(*p, workspace, reinterpret_cast<cudaStream_t>(stream));
+  MOS_CHECK_ARG(rc != MOS_EINVAL, "mos_lbfgs_solve: %s", solve_failure(rc));
+  return rc;
 }
 
 extern "C" int mos_lbfgs_solve_batch(const mos_lbfgs_problem* probs, int32_t n_probs, int32_t workers) {
@@ -392,7 +403,7 @@ extern "C" int mos_lbfgs_solve_batch(const mos_lbfgs_problem* probs, int32_t n_p
     ws_bytes = std::max(ws_bytes, Solver::workspace_bytes((long long)probs[i].out_f * probs[i].in_f,
                                                           probs[i].history > 0 ? probs[i].history : 25));
   const int nw = std::min<int>(workers, n_probs);
-  std::atomic<int> next(0), err(MOS_OK);
+  std::atomic<int> next(0), err(MOS_OK), failed(-1);   // failed: index of the first problem whose solve failed
   auto worker = [&]() {
     if (cudaSetDevice(dev) != cudaSuccess) {
       err = MOS_ECUDA;
@@ -409,7 +420,10 @@ extern "C" int mos_lbfgs_solve_batch(const mos_lbfgs_problem* probs, int32_t n_p
       const int j = next.fetch_add(1);
       if (j >= n_probs || err.load() != MOS_OK) break;
       const int rc = solve_one(probs[order[j]], ws, st);
-      if (rc != MOS_OK) err = rc;
+      if (rc != MOS_OK) {
+        int none = -1;
+        if (failed.compare_exchange_strong(none, order[j])) err = rc;
+      }
     }
     cudaStreamSynchronize(st);
     cudaFree(ws);
@@ -420,6 +434,8 @@ extern "C" int mos_lbfgs_solve_batch(const mos_lbfgs_problem* probs, int32_t n_p
   for (auto& t : threads) t.join();
   MOS_CHECK_CUDA(cudaDeviceSynchronize());
   const int rc = err.load();
-  MOS_CHECK_ARG(rc == MOS_OK, "mos_lbfgs_solve_batch: a solve failed with code %d (see mos_last_error of the first failure)", rc);
+  if (rc != MOS_OK)
+    return ::mos::set_err(rc, "mos_lbfgs_solve_batch: problem %d: %s", failed.load() >= 0 ? failed.load() : -1,
+                   failed.load() >= 0 ? solve_failure(rc) : "a worker could not create its stream or workspace");
   return MOS_OK;
 }

@@ -27,18 +27,25 @@ F32 = torch.float32
 
 
 # ------------------------------------------------------------------------------------------------ L-BFGS (restated)
+def _div(a, b):
+    """a / b with IEEE semantics (a signed infinity or NaN for b = 0, where Python raises), as csrc/lbfgs.cu divides"""
+    if b != 0 or b != b:
+        return a / b
+    return math.copysign(math.inf, a) * math.copysign(1.0, b) if a == a and a != 0 else math.nan
+
+
 def _cubic_min(x1, f1, g1, x2, f2, g2, bounds=None):
     """Minimiser of the cubic through (x1,f1,g1), (x2,f2,g2), clipped to `bounds` (Nocedal & Wright eq. 3.59)."""
     lo, hi = bounds if bounds is not None else ((x1, x2) if x1 <= x2 else (x2, x1))
-    d1 = g1 + g2 - 3.0 * (f1 - f2) / (x1 - x2)
+    d1 = g1 + g2 - _div(3.0 * (f1 - f2), x1 - x2)
     disc = d1 * d1 - g1 * g2
     if disc < 0:
         return 0.5 * (lo + hi)
     d2 = math.sqrt(disc)
     if x1 <= x2:
-        pos = x2 - (x2 - x1) * ((g2 + d2 - d1) / (g2 - g1 + 2.0 * d2))
+        pos = x2 - (x2 - x1) * _div(g2 + d2 - d1, g2 - g1 + 2.0 * d2)
     else:
-        pos = x1 - (x1 - x2) * ((g1 + d2 - d1) / (g1 - g2 + 2.0 * d2))
+        pos = x1 - (x1 - x2) * _div(g1 + d2 - d1, g1 - g2 + 2.0 * d2)
     return min(max(pos, lo), hi)
 
 
@@ -91,7 +98,7 @@ class _GramProblem:
         ops.ls_grad_loss(D, self.Y, self.R, self.s, self.f0, grad, self.loss64, self.scratch64)
         loss = self.loss64.item()
         self.evals += 1
-        if loss < self.best_loss:
+        if math.isfinite(loss) and loss < self.best_loss:        # as csrc/lbfgs.cu: a non-finite loss never qualifies
             self.best_loss = loss
             self.best_D = D.clone()
         return loss, grad
@@ -253,6 +260,8 @@ def solve_from_gram(G, Cm, vv, n_rows, W0, iters, native=None):
         D0 = torch.zeros(out_f * in_f, device=dev, dtype=F32)
         lbfgs_minimize(P, D0, iters)
         best_D = P.best_D
+        if best_D is None:
+            raise ValueError('solve_from_gram: no closure evaluation gave a finite loss (G or R holds NaN or Inf)')
     Wn = W0.clone()
     ops.vec_axpby(Wn.view(-1), best_D, 1.0, 1.0)
     return Wn

@@ -1,8 +1,11 @@
-"""Eager engine walks shared by the launch audits (test_gemm_engine_launches_gpu.py, test_attention_engine_launches_gpu.py).
+"""Eager engine walks shared by the launch audits (test_gemm_engine_launches_gpu.py, test_attention_engine_launches_gpu.py,
+test_norm_engine_launches_gpu.py, test_solver_engine_launches_gpu.py).
 
 Each walk builds its engine outside the audit and runs one engine call inside `audit()`, a zero-argument callable that
 returns the recorder's context manager.
 """
+import os
+
 import torch
 
 
@@ -143,3 +146,91 @@ def clip_text_and_train(audit, device):
         tr.forward_train(ids)
         tr.backward(dy)
     _run(audit, fwd_bwd)
+
+
+# ------------------------------------------------------------------------------------------------ gradient fusion
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'reference_golden.pt')
+
+
+def fusion_golden(audit):
+    """update_quasi_newton on both golden cases (K [30, 64] / [400, 48], 50 iterations) and merge_lora_into_weight on the
+    golden state dict"""
+    import gradient_fusion as gf
+    gold = torch.load(GOLDEN, weights_only=False)
+    g = gold['quasi_newton']
+    for case in ('', '2'):
+        _run(audit, lambda: gf.update_quasi_newton(g['K' + case], g['V' + case], g['W0' + case].clone(), 50, 'cuda'))
+    m = gold['merge_lora']
+    _run(audit, lambda: gf.merge_lora_into_weight(m['sd'], m['lora'], list(m['sd'].keys()), 'unet', m['alpha'], 'cuda'))
+
+
+def fusion_cross_kv(audit):
+    """merge_kv_in_cross_attention, 2 concepts x 6 text positions, K / V at the SD1.5 widths (320 / 640 / 1280 x 768)"""
+    import gradient_fusion as gf
+    g = torch.Generator().manual_seed(21)
+    names = [(0, 'down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight', 320),
+             (0, 'down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_v.weight', 320),
+             (1, 'down_blocks.1.attentions.0.transformer_blocks.0.attn2.to_k.weight', 640),
+             (2, 'mid_block.attentions.0.transformer_blocks.0.attn2.to_v.weight', 1280)]
+    sd = {n: torch.randn(c, 768, generator=g) * 768 ** -0.5 for _, n, c in names}
+    feats = [{i: torch.randn(6, 768, generator=g) for i in range(3)} for _ in range(2)]
+    tuned = []
+    for _ in range(2):
+        t = {}
+        for _, n, c in names:
+            dn = n.replace('.weight', '.lora_down.weight')
+            t[dn] = torch.randn(4, 768, generator=g) * 768 ** -0.5
+            t[dn.replace('lora_down', 'lora_up')] = torch.randn(c, 4, generator=g) * 0.1
+        tuned.append(t)
+    _run(audit, lambda: gf.merge_kv_in_cross_attention(sd, [(i, n) for i, n, _ in names], feats, tuned, [1.0, 0.7], 20))
+
+
+def fusion_text_encoder(audit):
+    """merge_text_encoder with two CLIPEncoderLayer LoRAs on a 2-layer CLIP (768 / 3072): gram_small at d = 3072"""
+    from transformers import CLIPTextConfig, CLIPTextModel
+    import gradient_fusion as gf
+    from oracle import inject
+    cfg = CLIPTextConfig(vocab_size=1000, hidden_size=768, intermediate_size=3072, num_hidden_layers=2,
+                         num_attention_heads=12, max_position_embeddings=77, eos_token_id=999, bos_token_id=998,
+                         pad_token_id=999)
+    torch.manual_seed(0)
+    base = CLIPTextModel(cfg).eval()
+    sd = {k: v.clone() for k, v in base.state_dict().items()}
+    loras = [inject.random_lora_state(base, seed=40 + c, where='CLIPEncoderLayer', up_std=0.05) for c in range(2)]
+    g = torch.Generator().manual_seed(9)
+    prompts = [[torch.cat([torch.tensor([998]), torch.randint(0, 990, (n,), generator=g), torch.tensor([999])])
+                for n in (5, 2, 5, 2)] for _ in range(2)]
+    _run(audit, lambda: gf.merge_text_encoder(sd, loras, [1.0, 0.7], prompts, 10, pad_id=999))
+
+
+def fusion_spatial_whole_block_tiny(audit):
+    """merge_spatial_attention on the tiny topology with two Transformer2DModel LoRAs (2 sampling steps, 5 iterations):
+    the Gram recorder's transposes of strided activations, sgemm at in = 4C (ff.net.2), 4-D proj_in / proj_out"""
+    import gradient_fusion as gf
+    from oracle import inject
+    from oracle import unet as ou
+    u0 = ou.build_unet(0, ou.TINY)
+    sd = {k: v.clone() for k, v in u0.state_dict().items()}
+    loras = [inject.random_lora_state(u0, seed=10 + c, where='Transformer2DModel', up_std=0.05) for c in range(2)]
+    spatial = [{k: v for k, v in l.items() if 'attn2.to_k' not in k and 'attn2.to_v' not in k} for l in loras]
+    embeds = [torch.randn(1, 16, 77, 768, generator=torch.Generator().manual_seed(20 + c)) for c in range(2)]
+    _run(audit, lambda: gf.merge_spatial_attention(sd, spatial, [1.0, 1.0], embeds, 5, latent_hw=(16, 16),
+                                                   num_inference_steps=2, seed=0,
+                                                   block_out=ou.TINY['block_out_channels'], layers=1))
+
+
+def fusion_sd15_solves(audit, iters=3):
+    """the two largest SD1.5 solves of a whole-block fusion, ff.net.0.proj [10240, 1280] and ff.net.2 [1280, 5120]
+    (13.1 M-element vectors, a 5120^2 Gram matrix), from Gram matrices of 6000 random feature rows"""
+    import gradient_fusion as gf
+    jobs = []
+    for name, out_f, in_f in (('ff.net.0.proj', 10240, 1280), ('ff.net.2', 1280, 5120)):
+        g = torch.Generator(device='cuda').manual_seed(out_f)
+        X = torch.randn(6000, in_f, device='cuda', generator=g)
+        W0 = torch.randn(out_f, in_f, device='cuda', generator=g) * in_f ** -0.5
+        Wt = W0 + 0.01 * torch.randn(out_f, in_f, device='cuda', generator=g)
+        G = X.t() @ X
+        Cm = Wt @ G
+        vv = float((Wt.double() * (Wt.double() @ G.double())).sum())
+        jobs.append((name, G, Cm, vv, 6000, W0, (out_f, in_f)))
+    return _run(audit, lambda: gf.solve_all(jobs, iters))

@@ -119,7 +119,8 @@ def test_native_lbfgs_driver_bit_identical_to_python_driver(cuda, out_f, in_f, n
 
 
 def test_dgemm_mixed_tilings(cuda):
-    """the fp64 closure product in both tilings (32- and 64-row CTA tiles) vs torch fp64"""
+    """the fp64 closure product in the default 64 x 64 tiling vs torch fp64 (MOS_DGEMM_TILE is read once per process;
+    test_solver_engine_launches_gpu.py runs the 32 x 64 and 64 x 128 tiles in child processes)"""
     from mos_b200 import ops
     for M, K, N in ((320, 768, 768), (1280, 1280, 1280), (100, 70, 130)):
         A = torch.randn(M, K, device=cuda)
