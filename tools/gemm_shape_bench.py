@@ -11,14 +11,19 @@ the first work item of the first 8 CTAs (medians over the CTAs that stamped both
   stage  -> staging tile written                   wake   -> the producer observed epi_full
   issue  -> TMA stores issued                      drain  -> the stores have read the staging tile
   epi    accumulators ready -> tile written (ops + rdy + stage + wake + issue + drain)
-and `epi2`, the same epilogue phase of the second work item in CTAs that run several.  A CTA with several tiles writes
+and `epi2`, the same epilogue phase of the second work item in CTAs that run several.  `cyc/kb` is the mainloop per k
+block in SM cycles at the bound clock (640 at the tensor rate), and `opMB` the operand bytes the launch moves from L2
+into shared memory (items x k blocks x stage bytes).  A CTA with several tiles writes
 a tile out only after issuing the next tile's k blocks, so there `epi` includes that wait.  On the copy-out path (no
 TMA stores) the consumers write the tile and `wake`, `issue` and `drain` are empty.
 
 The replay calls ops.gemm, which encodes the tensor maps on the host at every launch: a launch shorter than that host
 work is timed at the host's rate, so compare short launches against the bound with the timeline's phases.
 
-    python tools/gemm_shape_bench.py [--reps 50] [--out DIR]
+    python tools/gemm_shape_bench.py [--reps 50] [--max-ctas N] [--out DIR]
+
+--max-ctas caps the persistent grid (MOS_GEMM_MAX_CTAS): a k block that gets faster when fewer SMs run is contending
+for a resource the SMs share (L2 bandwidth), not bound inside the SM.
 """
 import argparse
 import ctypes
@@ -34,6 +39,7 @@ for p in (ROOT, os.path.join(ROOT, 'mix-of-show_b200')):
 
 BM, BN, BK = 128, 160, 64
 CYCLES_PER_KBLOCK = BM * BN * BK * 2 // 4096     # 640
+A_STAGE_BYTES, B_STAGE_BYTES, LORA_STAGE_BYTES = BM * BK * 2, BN * BK * 2, 16 * BK * 2
 
 
 def conv_m_tiles(B, H, Wd):
@@ -112,7 +118,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--reps', type=int, default=50, help='timed launches per shape (after 5 warm-up launches)')
     ap.add_argument('--out', default=None, help='also write the table as DIR/gemm_shapes.json')
+    ap.add_argument('--max-ctas', type=int, default=0, help='cap the persistent grid at N CTAs (MOS_GEMM_MAX_CTAS)')
     args = ap.parse_args()
+    if args.max_ctas > 0:
+        os.environ['MOS_GEMM_MAX_CTAS'] = str(args.max_ctas)     # read once, at the first launch
     import torch
     assert torch.cuda.is_available(), 'gemm_shape_bench.py needs a GPU'
     import bench
@@ -189,30 +198,37 @@ def main():
             return v[len(v) // 2] if v else float('nan')
 
         bound_us = math.ceil(items / n_sm) * kbi * CYCLES_PER_KBLOCK / (clk_ghz * 1e3)
-        rows.append(dict(M=M, N=N, K=K, kind=label, count=len(calls_g), items=items, kb_per_item=kbi, us=us,
+        stage = A_STAGE_BYTES + B_STAGE_BYTES + (LORA_STAGE_BYTES if kw.get('lora_down') is not None else 0)
+        main_us = med(3, 4)
+        rows.append(dict(cycles_per_kb=main_us * clk_ghz * 1e3 / kbi, operand_mb=items * kbi * stage / 1e6,
+                         M=M, N=N, K=K, kind=label, count=len(calls_g), items=items, kb_per_item=kbi, us=us,
                          tflops=flops / (us * 1e-6) / 1e12, bound_us=bound_us,
-                         first_tma_us=med(1, 3), mainloop_us=med(3, 4), epilogue_us=med(4, 5),
+                         first_tma_us=med(1, 3), mainloop_us=main_us, epilogue_us=med(4, 5),
                          ops_us=med(4, 6), ready_us=med(6, 7), stage_us=med(7, 8), wake_us=med(8, 9),
                          issue_us=med(9, 10), drain_us=med(10, 5), epilogue2_us=med(11, 15)))
     rows.sort(key=lambda r: -r['us'] * r['count'])
-    print(f"card: {info}  SMs {n_sm}  bound clock {clk_ghz:.3f} GHz  launches/step {len(calls)}")
+    print(f"card: {info}  SMs {n_sm}  grid cap {args.max_ctas or n_sm}  bound clock {clk_ghz:.3f} GHz  "
+          f"launches/step {len(calls)}")
     hdr = (f"{'M':>6} {'N':>5} {'K':>5} {'kind':<18} {'n':>3} {'items':>5} {'kb':>4} {'us':>8} {'TF/s':>6} "
            f"{'bound':>7} {'tma1':>6} {'main':>7} {'epi':>6} {'ops':>6} {'rdy':>6} {'stage':>6} {'wake':>6} "
-           f"{'issue':>6} {'drain':>6} {'epi2':>6}")
+           f"{'issue':>6} {'drain':>6} {'epi2':>6} {'cyc/kb':>7} {'opMB':>7}")
     print(hdr)
     for r in rows:
         print(f"{r['M']:>6} {r['N']:>5} {r['K']:>5} {r['kind']:<18} {r['count']:>3} {r['items']:>5} "
               f"{r['kb_per_item']:>4} {r['us']:>8.2f} {r['tflops']:>6.1f} {r['bound_us']:>7.2f} "
               f"{r['first_tma_us']:>6.2f} {r['mainloop_us']:>7.2f} {r['epilogue_us']:>6.2f} {r['ops_us']:>6.2f} "
               f"{r['ready_us']:>6.2f} {r['stage_us']:>6.2f} {r['wake_us']:>6.2f} {r['issue_us']:>6.2f} "
-              f"{r['drain_us']:>6.2f} {r['epilogue2_us']:>6.2f}")
+              f"{r['drain_us']:>6.2f} {r['epilogue2_us']:>6.2f} {r['cycles_per_kb']:>7.0f} {r['operand_mb']:>7.1f}")
     tot = sum(r['us'] * r['count'] for r in rows)
     bnd = sum(r['bound_us'] * r['count'] for r in rows)
-    print(f"step total: {tot / 1e3:.3f} ms of back-to-back launches, tensor-rate bound {bnd / 1e3:.3f} ms")
+    opb = sum(r['operand_mb'] * r['count'] for r in rows)
+    print(f"step total: {tot / 1e3:.3f} ms of back-to-back launches, tensor-rate bound {bnd / 1e3:.3f} ms, "
+          f"operand bytes {opb / 1e3:.2f} GB")
     if args.out:
         os.makedirs(args.out, exist_ok=True)
         with open(os.path.join(args.out, 'gemm_shapes.json'), 'w') as f:
-            json.dump({'card': info, 'rows': rows, 'total_ms': tot / 1e3, 'bound_ms': bnd / 1e3}, f, indent=1)
+            json.dump({'card': info, 'max_ctas': args.max_ctas or n_sm, 'rows': rows, 'total_ms': tot / 1e3,
+                       'bound_ms': bnd / 1e3, 'operand_gb': opb / 1e3}, f, indent=1)
 
 
 if __name__ == '__main__':
