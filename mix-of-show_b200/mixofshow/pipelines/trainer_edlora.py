@@ -24,6 +24,9 @@ from mos_b200.clip_train_engine import CLIP_WHERE
 from mos_b200.engine import ehs_to_layer_major
 from mos_b200.train_engine import UNET_WHERE, TrainEngine
 
+VANILLA_LORA_UNSUPPORTED = ('enable_edlora=False (vanilla LoRA with one embedding per concept) is not built on the GPU '
+                            'path: the cross-attention kernels take layer-wise embeddings')
+
 
 def _check_where(where, allowed, part):
     if where not in allowed:
@@ -183,8 +186,7 @@ class EDLoRATrainer:
                  seed=0):
         from mixofshow.utils import model_io
         if not enable_edlora:
-            raise NotImplementedError('enable_edlora=False (vanilla LoRA with one embedding per concept) is not built on '
-                                      'the GPU path: the cross-attention kernels take layer-wise embeddings')
+            raise NotImplementedError(VANILLA_LORA_UNSUPPORTED)
         self.device = torch.device(device)
         self.enable_edlora = True
         self.unet = model_io.load_unet(pretrained_path)                               # :44

@@ -13,7 +13,12 @@ Data: the image pipeline (LoraDataset transforms, VAE encoder) is outside the ho
 `datasets.train` is read as a `LatentDataset`: `path` = a torch file {'latents' [n,4,h,w] (VAE latents x 0.18215),
 'prompts' [n str], 'masks' [n,1,h,w], optional 'img_masks'}; `replace_mapping`, `batch_size_per_gpu` and
 `dataset_enlarge_ratio` keep their reference meaning.
+
+Checkpoints and validation (train_edlora.py:157-189): `edlora_model-{step}.pth` every `logger.save_checkpoint_freq` steps
+and `edlora_model-latest.pth` at the end; with `val.val_during_save`, each saved checkpoint is sampled over
+`datasets.val_vis` for every alpha of `val.alpha_list` by test_edlora.py's `visual_validation`, sharded across ranks.
 """
+import functools
 import os
 
 import torch
@@ -33,10 +38,11 @@ def linear_lr(base_lr, step, num_training_steps):
 
 
 def train(trainer, batches, *, dataset_len, batch_size_per_gpu, gradient_accumulation_steps=1, print_freq=0,
-          log=print, emb_norm_threshold=5.5e-1):
+          log=print, emb_norm_threshold=5.5e-1, save_checkpoint_freq=0, save=None):
     """Runs the loop of train_edlora.py:105-158; returns the list of per-step mean losses (rank-averaged).
     `batches`: dicts with either ('images' = latents, 'prompts', 'masks', 'img_masks') for EDLoRATrainer or ('latents',
-    'encoder_hidden_states', 'masks', 'img_masks'[, 'text_input_ids']) for UNetLoRATrainer."""
+    'encoder_hidden_states', 'masks', 'img_masks'[, 'text_input_ids']) for UNetLoRATrainer.  `save(global_step)` is
+    called after every `save_checkpoint_freq`-th optimiser step (train_edlora.py:157-158)."""
     world = dist.get_world_size() if dist.is_initialized() else 1
     total_iter = total_iterations(dataset_len, batch_size_per_gpu, world, gradient_accumulation_steps)
     sched_steps = total_iter * gradient_accumulation_steps
@@ -78,6 +84,8 @@ def train(trainer, batches, *, dataset_len, batch_size_per_gpu, gradient_accumul
             if print_freq and global_step % print_freq == 0:
                 extra = '' if norm_mean is None else f' Norm_mean {norm_mean:.4f}'
                 log(f'iter {global_step}: loss {mean_loss:.5f} lr {state.lrs[2]:.3e}{extra}')
+            if save is not None and save_checkpoint_freq and global_step % save_checkpoint_freq == 0:
+                save(global_step)
         sched_k += 1
     return losses
 
@@ -145,20 +153,49 @@ def main(argv=None):
     accum = int(opt.get('gradient_accumulation_steps', 1))
     log = print if rank == 0 else (lambda *a, **k: None)
     log(f'***** Running training *****  examples {len(dataset)}, batch/GPU {bs}, world {world}, accumulation {accum}')
+    name = opt.get('name', 'edlora')
+    paths = dict(opt.get('path') or {})
+    paths['models'] = paths.get('models') or os.path.join('experiments', name, 'models')
+    paths['visualization'] = paths.get('visualization') or os.path.join('experiments', name, 'visualization')
+    val_opt = opt.get('val') or {}
+    val_dataset = None
+    if val_opt.get('val_during_save'):
+        from mixofshow.data.prompt_dataset import PromptDataset
+        val_dataset = PromptDataset(opt['datasets']['val_vis'])
+    save = functools.partial(save_and_validation, trainer, dict(opt, path=paths), val_dataset, rank=rank, world=world,
+                             log=log)
     losses = train(trainer, dataset.batches(bs, rank, world, seed=(seed or 0)), dataset_len=len(dataset),
                    batch_size_per_gpu=bs, gradient_accumulation_steps=accum,
                    print_freq=int(opt.get('logger', {}).get('print_freq', 10)), log=log,
-                   emb_norm_threshold=float(train_opt.get('emb_norm_threshold', 5.5e-1)))
-    if rank == 0:                                                                           # train_edlora.py:161-171
-        out_dir = (opt.get('path') or {}).get('models') or os.path.join('experiments', opt.get('name', 'edlora'), 'models')
-        os.makedirs(out_dir, exist_ok=True)
-        save_path = os.path.join(out_dir, 'edlora_model-latest.pth')
+                   emb_norm_threshold=float(train_opt.get('emb_norm_threshold', 5.5e-1)),
+                   save_checkpoint_freq=int((opt.get('logger') or {}).get('save_checkpoint_freq', 0)), save=save)
+    save('latest')
+    if world > 1:
+        dist.destroy_process_group()
+    return losses
+
+
+def save_and_validation(trainer, opt, val_dataset, global_step, *, rank=0, world=1, log=print):
+    """train_edlora.py:165-189: rank 0 writes `edlora_model-{global_step}.pth`; then every rank waits for it and, when
+    `val_dataset` is given, samples its share of the set from that file for each alpha of `val.alpha_list` into
+    `Iters-{global_step}_Alpha-{alpha}` (test_edlora.py's `visual_validation`).  The pipeline is loaded fresh from the
+    pretrained directory and the checkpoint file, so validation reads nothing of the trainer."""
+    save_path = os.path.join(opt['path']['models'], f'edlora_model-{global_step}.pth')
+    if rank == 0:
+        os.makedirs(opt['path']['models'], exist_ok=True)
         torch.save({'params': trainer.delta_state_dict()}, save_path)
         log(f'Save state to {save_path}')
     if world > 1:
         dist.barrier()
-        dist.destroy_process_group()
-    return losses
+    if val_dataset is None:
+        return
+    import test_edlora
+    log(f'Start validation {save_path}:')
+    for alpha in test_edlora.alpha_list(opt):
+        pipe = test_edlora.load_pipeline(opt['models']['pretrained_path'], save_path, alpha)
+        test_edlora.visual_validation(pipe, val_dataset, f'Iters-{global_step}_Alpha-{alpha}', opt, rank, world)
+        del pipe
+        test_edlora.free_pipeline()
 
 
 if __name__ == '__main__':
