@@ -2,7 +2,9 @@
 test_norm_engine_launches_gpu.py, test_solver_engine_launches_gpu.py).
 
 Each walk builds its engine outside the audit and runs one engine call inside `audit()`, a zero-argument callable that
-returns the recorder's context manager.
+returns the recorder's context manager.  The product-shape walks (train_sd15_full, validation_sd15) build through
+bench.py's workload and are built the same way by test_graph_replay_gpu.py, which holds the captured graphs bit-identical
+to these eager walks.
 """
 import os
 
@@ -88,6 +90,118 @@ def train_sd15_channels_whole_block(audit, attn_reg_weight=None, optimizer_step=
         packed = [e[k] for e in eng.w.values() if isinstance(e, dict) for k in ('lora_down', 'lora_up')
                   if isinstance(e.get(k), torch.Tensor)]
         _run(audit, eng.optimizer_step, register=[eng.state.params, *eng._lora_keep, *packed])
+
+
+def build_train_sd15_full(use_graph=True):
+    """The training step of bench.py `train_leg` at B = 2 (the shipped configs' batch_size_per_gpu): SD1.5 UNet at 64 x 64
+    with a rank-4 `where: Attention` LoRA, the attention regulariser on all 16 cross layers (weight 0.01,
+    reg_full_identity=False) and a 12-layer CLIPTrainEngine over 16 * B layer-major sequences attached (text_grad), all in
+    one shared dp.FlatTrainState.  -> SimpleNamespace(eng, text, state, B, nx, concept_ids)"""
+    import math
+    from types import SimpleNamespace
+
+    from mos_b200 import dp
+    from mos_b200.clip_train_engine import CLIPTrainEngine
+    from mos_b200.train_engine import TrainEngine
+    import bench
+    sd, lora, _, _, _ = bench.build_workload()
+    B, dev = 2, torch.device('cuda')
+    tsd = bench.synthetic_clip_state()
+    g0 = torch.Generator().manual_seed(12)
+    tlora = {}                                      # the CLIPAttention LoRA train_leg builds
+    for i in range(12):
+        for pj in ('q_proj', 'k_proj', 'v_proj', 'out_proj'):
+            m = f'text_model.encoder.layers.{i}.self_attn.{pj}'
+            tlora[m + '.lora_down.weight'] = (torch.rand(4, 768, generator=g0) * 2 - 1) / math.sqrt(768)
+            tlora[m + '.lora_up.weight'] = torch.randn(768, 4, generator=g0) * 0.02
+    concept_ids = list(range(49408, 49408 + 32))
+    n_text = CLIPTrainEngine.lora_param_count(12, 768, 960)
+    n_unet = sum(v.numel() for v in lora.values())
+    state = dp.FlatTrainState(len(concept_ids), 768, n_text, n_unet, lrs=(1e-3, 1e-5, 1e-4), device=dev)
+    eng = TrainEngine(sd, B, 64, 64, lora=lora, attn_reg_weight=0.01, reg_full_identity=False, state=state,
+                      state_offset=state.group_end[1], text_grad=True, device=dev, use_graph=use_graph)
+    nx = len(eng.xattn_names)
+    text = CLIPTrainEngine(tsd, nx * B, lora=tlora, lora_alpha=1.0, concept_token_ids=concept_ids, state=state,
+                           emb_offset=0, lora_offset=state.group_end[0], device=dev)
+    eng.attach_text_engine(text)
+    return SimpleNamespace(eng=eng, text=text, state=state, B=B, nx=nx, concept_ids=concept_ids)
+
+
+def train_sd15_full_inputs(w, seed):
+    """one batch of the bench leg's kind: x0, noise, t, box masks and layer-major token ids [16 * B, 77] (BOS, 8 words with
+    the two concept tokens of each layer at positions 2 and 3, EOS padding); the box moves with the seed"""
+    B, nx = w.B, w.nx
+    g = torch.Generator().manual_seed(seed)
+    x0 = torch.randn(B, 4, 64, 64, generator=g).cuda()
+    noise = torch.randn(B, 4, 64, 64, generator=g).cuda()
+    t = torch.randint(0, 1000, (B,), generator=g).cuda()
+    ids = torch.randint(1000, 40000, (nx, B, 77), generator=g)
+    ids[:, :, 0] = 49406
+    ids[:, :, 9:] = 49407
+    for l in range(nx):
+        ids[l, :, 2], ids[l, :, 3] = w.concept_ids[l % 16], w.concept_ids[16 + l % 16]
+    r0, c0 = (int(v) for v in torch.randint(0, 17, (2,), generator=g))
+    masks = torch.zeros(B, 1, 64, 64)
+    masks[:, :, r0:r0 + 48, c0:c0 + 32] = 1.0
+    return dict(latents=x0, noise=noise, timesteps=t, ehs_layers=None, masks=masks.cuda(), token_pos=[[2, 3]] * B,
+                text_ids=ids.reshape(nx * B, 77))
+
+
+def train_optimizer_step(w):
+    """the bench leg's optimiser step: the loss onto the flat buffer, flat AdamW, both LoRA re-packs"""
+    from mos_b200 import dp
+    scale = dp.allreduce_flat_device(w.state, w.eng.loss_out[0:1])
+    dp.optimizer_step(w.state, scale)
+    w.eng.refresh_lora()
+    w.text.refresh_lora()
+
+
+def _packed_lora(ents):
+    return [e[k] for e in ents if isinstance(e, dict) for k in ('lora_down', 'lora_up')
+            if isinstance(e.get(k), torch.Tensor)]
+
+
+def train_sd15_full(audit):
+    """bench.py `train_leg` at B = 2, eager: one forward_backward (CLIP forward, UNet forward at 64 x 64, masked MSE, the
+    regulariser at 64^2 / 32^2 / 16^2 / 8^2, UNet backward with d(text embeddings), CLIP backward), then the optimiser step
+    (its lora_pack tables point into the flat state and both engines' GEMM operands, registered with the audit)"""
+    w = build_train_sd15_full(use_graph=False)
+    batch = train_sd15_full_inputs(w, 100)
+    _run(audit, lambda: w.eng.forward_backward(**batch))
+    text_ents = [v for ent in w.text.w.values() for v in ent.values()]
+    _run(audit, lambda: train_optimizer_step(w),
+         register=[w.state.params, *w.eng._lora_keep, *w.text._keep, *_packed_lora(w.eng.w.values()),
+                   *_packed_lora(text_ents)])
+    return w
+
+
+def build_validation_sd15():
+    """bench.build_workload(images=4) in bench.build_pipeline: the 4-prompt validation call of the SD1.5 UNet (CFG batch 8)
+    -> (pipe, cond [4, 16, 77, 768], neg [4, 77, 768], latents [4, 4, 64, 64])"""
+    import bench
+    sd, lora, lat, ehs, cfg = bench.build_workload(images=4)
+    pipe = bench.build_pipeline(sd, lora, cfg, torch.device('cuda'))
+    return pipe, ehs[4:], ehs[:4, 0], lat
+
+
+def validation_call(pipe, cond, neg, lat, steps=2, callback=None):
+    return pipe(prompt_embeds=cond.cuda(), negative_prompt_embeds=neg.cuda(), latents=lat.clone(),
+                num_inference_steps=steps, guidance_scale=7.5, output_type='latent', callback=callback).images
+
+
+def validation_sd15(audit):
+    """the validation pass at SD1.5 size: a 4-prompt CFG call (UNet batch 8, 2 DPM-Solver++ steps, eager UNet, latent
+    output), then an SD1.5-width VAEEngine decode of 4 latents to 512 x 512"""
+    from mos_b200.vae_engine import VAEEngine
+    from oracle import vae as ov
+    pipe, cond, neg, lat = build_validation_sd15()
+    pipe.unet.use_graph = False
+    out = _run(audit, lambda: validation_call(pipe, cond, neg, lat))
+    del pipe
+    ref = ov.build_vae(0, None)
+    sd = {k: v.detach().clone() for k, v in ref.state_dict().items()}
+    eng = VAEEngine(sd, 4, 512, 512, block_out=ov.SD15_VAE['block_out_channels'], layers=ov.SD15_VAE['layers_per_block'])
+    _run(audit, lambda: eng.decode(out / 0.18215))
 
 
 def vae_512(audit):

@@ -10,7 +10,10 @@ The end-to-end tests compare one global rel-L2 or LoRA gradients at 8e-2: one wr
   drop-in RegionT2I_AttnProcessor (mos_b200/functional.py) on a 12 x 24 feature map with 3 regions;
 - bf16 training at the SD1.5 widths, 16 x 16, B = 2, with the attention regulariser (pcols, pos, gcols);
 - CLIP: CLIPTextEngine (causal forward), CLIPTrainEngine forward + backward (causal lse2, causal backward, dq | dk | dv
-  thirds of one storage).
+  thirds of one storage);
+- the product's training step (bench.py train_leg at B = 2): bf16 SD1.5 at 64 x 64 (4096 / 1024 / 256 / 64 tokens) with
+  the regulariser on all 16 cross layers and the 12-layer CLIP encoder over 32 sequences;
+- the product's validation pass: a 4-prompt CFG call (UNet batch 8: B H = 64) and the VAE decode of its 4 latents.
 The last test prints one row per path key and requires the keys reached to be exactly PATH_KEYS.
 """
 import time
@@ -33,6 +36,10 @@ pytestmark = pytest.mark.gpu
 #     fwd|bf16 / bwd|bf16 / delta / transpose at 256 / 64 / 16 / 4 tokens;
 #   clip_engine.py forward and clip_train_engine.py forward_train (attention_causal, without and with lse2), backward
 #     (heads_transpose, attn_delta, causal attention_bwd into the dqkv thirds): the D=80 causal keys.
+# Only the product walks (train_sd15_full, validation_sd15) reach the keys marked "product": the toy training walk has
+# d = 80 / 160 only at 64 / 16 / 4 tokens (query tails), the 64 x 64 step at 1024 (d = 80) and 256 / 64 (d = 160) tokens,
+# so the d = 80 / 160 self-attention forward and backward run tail-free multi-tile launches, the cross-attention full
+# query tiles, and the 64-token d = 160 backward a one-tile launch with a query tail but no key tail.
 PATH_KEYS = {
     # UNetEngine, fp16
     'fwd|fp16|D=40|multi',
@@ -53,15 +60,24 @@ PATH_KEYS = {
     # TrainEngine, bf16
     'fwd|bf16|D=40|multi|lse2',
     'fwd|bf16|D=40|one|lse2|pcols|ktail',
+    'fwd|bf16|D=80|multi|lse2',                     # product
+    'fwd|bf16|D=80|multi|lse2|pcols|ktail',         # product
     'fwd|bf16|D=80|multi|lse2|qtail|ktail',
     'fwd|bf16|D=80|multi|lse2|pcols|qtail|ktail',
     'fwd|bf16|D=160|one|lse2|qtail|ktail',
+    'fwd|bf16|D=160|multi|lse2',                    # product
+    'fwd|bf16|D=160|one|lse2|pcols|ktail',          # product
     'fwd|bf16|D=160|one|lse2|pcols|qtail|ktail',
     'bwd|bf16|D=40|multi',
     'bwd|bf16|D=40|multi|gcols|ktail',
     'bwd|bf16|D=80|one|qtail',
+    'bwd|bf16|D=80|multi',                          # product
+    'bwd|bf16|D=80|multi|gcols|ktail',              # product
     'bwd|bf16|D=80|multi|gcols|qtail|ktail',
     'bwd|bf16|D=160|one|qtail|ktail',
+    'bwd|bf16|D=160|one|qtail',                     # product
+    'bwd|bf16|D=160|multi',                         # product
+    'bwd|bf16|D=160|multi|gcols|ktail',             # product
     'bwd|bf16|D=160|multi|gcols|qtail|ktail',
     'delta|D=40',
     'delta|D=40|pcols',
@@ -131,6 +147,14 @@ def test_train_with_attention_regulariser(cuda):
 
 def test_clip_text_and_train(cuda):
     walks.clip_text_and_train(_audit, cuda)
+
+
+def test_train_sd15_full(cuda):
+    walks.train_sd15_full(_audit)
+
+
+def test_validation_sd15(cuda):
+    walks.validation_sd15(_audit)
 
 
 def test_coverage_table(cuda):

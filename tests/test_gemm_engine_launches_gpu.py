@@ -9,6 +9,10 @@ write into a Q/K pad column all vanish inside their eps / gradient bounds.  The 
 - CLIP: CLIPTextEngine, 12 layers, fused CLIPAttention LoRA; CLIPTrainEngine forward + backward, CLIPEncoderLayer LoRA;
 - VAE encode + decode at 512 x 512, B = 1;
 - gradient fusion: Gram recording of one spatial stage with whole-block keys;
+- the product's training step (bench.py train_leg at B = 2): SD1.5 UNet at 64 x 64 with an Attention LoRA, the regulariser
+  on all 16 cross layers, the 12-layer CLIP encoder trained in the same step (d(text embeddings) GEMMs, CLIP backward from
+  the UNet's pitched d_ehs), then the optimiser step;
+- the product's validation pass: a 4-prompt CFG call (UNet batch 8, 2 steps) and the VAE decode of its 4 latents at 512;
 - the opt-in paths: a child process repeats the 64 x 64 walk with MOS_SPLITK_FUSED=1 MOS_L2_PREFETCH=1 (both read at
   import); its launches are audited too, and its eps must be bit-identical to the default walk's (the in-kernel finalize
   sums the partials in the same order as mos_splitk_finalize).
@@ -40,6 +44,10 @@ pytestmark = pytest.mark.gpu
 # the 4 x 4 / 2 x 2 levels of a 16 x 16 training latent); partial and splitk_finalize are the split-K launches of
 # UNetEngine.gemm (fused: MOS_SPLITK_FUSED=1); rows / rows+res_smem are every other linear and conv.  No engine launch
 # reaches the global-memory residual or copied-out row output.
+# Only the product walks (train_sd15_full, validation_sd15) reach the keys marked "product": at 64 x 64 (M = 8192) the
+# training convs have enough tiles to skip split-K (UNetEngine._splits), so conv1 stores directly with the time-embedding
+# batch bias (train_engine.py:290), conv2 with the staged residual (:293), and so do the backward convs (:303 / :308 /
+# :658; :303 and :658 read dOut at a pitched lda); the attn1 q | k | v projections write 4096 / 1024 tokens through the bf16 head-split TMA path.
 PATH_KEYS = {
     'f32+acc|global|fp16',
     'f32|global|fp16',
@@ -63,7 +71,9 @@ PATH_KEYS = {
     'heads|copy|bf16|lora|T=4',
     'heads|copy|bf16|lora|T=77',
     'heads|copy|fp16|lora|T=288',
+    'heads|tma|bf16|lora|T=1024',                  # product
     'heads|tma|bf16|lora|T=256',
+    'heads|tma|bf16|lora|T=4096',                  # product
     'heads|tma|bf16|lora|T=64',
     'heads|tma|fp16|T=256',
     'heads|tma|fp16|T=64',
@@ -81,11 +91,14 @@ PATH_KEYS = {
     'partial|global|fp16|conv|fused',
     'partial|global|fp16|fused',
     'rows+res_smem|tma|bf16',
+    'rows+res_smem|tma|bf16|conv',                 # product
     'rows+res_smem|tma|bf16|lora',
     'rows+res_smem|tma|fp16',
     'rows+res_smem|tma|fp16|conv',
     'rows+res_smem|tma|fp16|lora',
     'rows|tma|bf16',
+    'rows|tma|bf16|conv',                          # product
+    'rows|tma|bf16|conv|bb',                       # product
     'rows|tma|bf16|lora',
     'rows|tma|fp16',
     'rows|tma|fp16|conv',
@@ -170,6 +183,14 @@ def test_opt_in_paths_child(cuda, tmp_path):
     assert 'default' in EPS
     assert torch.equal(eps.view(torch.int32), EPS['default'].cpu().view(torch.int32)), \
         'the in-kernel split-K finalize changed eps'
+
+
+def test_train_sd15_full(cuda):
+    walks.train_sd15_full(lambda: ga.Recorder(STATS))
+
+
+def test_validation_sd15(cuda):
+    walks.validation_sd15(lambda: ga.Recorder(STATS))
 
 
 def test_coverage_table(cuda):

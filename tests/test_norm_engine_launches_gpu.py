@@ -5,8 +5,11 @@ GroupNorm workspace prefix), unchanged operands and a bit-identical second launc
 The walks are the eager walks of the other launch audits (tests/engine_walks.py): fp16 sampling at 64 x 64 (plain, and
 a regional step with 3 boxes and emit_probs), at 96 x 192 with a whole-block LoRA, the drop-in RegionT2I_AttnProcessor,
 bf16 training at the SD1.5 widths with the attention regulariser followed by the optimiser step, CLIP text encoding and
-training, the VAE at 512 x 512 and the EDLoRAPipeline sampling loop (3 steps, CFG).  The last test
-prints one row per path key and requires the keys reached to be exactly PATH_KEYS.
+training, the VAE at 512 x 512 and the EDLoRAPipeline sampling loop (3 steps, CFG); and the product's own shapes: the
+training step of bench.py train_leg at B = 2 (SD1.5 at 64 x 64, regulariser on all 16 cross layers without full_identity,
+the 12-layer CLIP encoder trained in the same step, then AdamW and the LoRA re-pack over the three-group flat state) and
+the validation pass (a 4-prompt CFG call, UNet batch 8, and the VAE decode of its 4 latents).  The last test prints one
+row per path key and requires the keys reached to be exactly PATH_KEYS.
 """
 import time
 
@@ -20,7 +23,7 @@ pytestmark = pytest.mark.gpu
 
 # The path keys (norm_audit.norm_path) the walks reach on a 132-SM H100 (the GroupNorm cluster width k depends on the SM
 # count through the 2 * SMs minimum grid), by engine call site:
-#   engine.py:347 groupnorm (UNet, fp16 sampling / bf16 training): the cluster kernel at k = 1 / 4 / 8, vec 2 / 4;
+#   engine.py:347 groupnorm (UNet, fp16 sampling / bf16 training): the cluster kernel at k = 1 / 2 / 4 / 8, vec 2 / 4;
 #     vae_engine.py:161 at 512 x 512: the two-launch fallback with its partial workspace;
 #   engine.py:355 / clip_train_engine.py:293 layernorm: C = 320 / 640 / 1280 and 768 (CLIP); the pipeline's CLIP
 #     encoder runs 2 x 77 = 154 rows, a tail of the 8-row block;
@@ -35,13 +38,19 @@ pytestmark = pytest.mark.gpu
 #   engine.py:513 _region_rewrite and functional.py:162: region_combine in place over 3 regions;
 #   train_engine.py: upsample2x, im2col pad 1, add_rows, geglu, upsample2x_bwd, col2im, conv_out_bwd, add_noise;
 #   clip_engine.py / clip_train_engine.py: clip_embed, clip_embed_bwd, quick_gelu (in place), quick_gelu_fwd / _bwd.
+# Only the product walks (train_sd15_full, validation_sd15) reach the keys marked "product": the regulariser without
+# full_identity (train_engine.py:601, groups of 5 layers at 64^2 / 32^2 / 16^2 and the mid layer alone at 8^2), the
+# time-MLP gemv at batch 8, GroupNorm at k = 2 (fp16, B = 8) and k = 8 / vec 4 (bf16 at 64 x 64), and lora_grad at
+# R = 32 (CLIP, 32 x 77 rows) and R = 64 (UNet, 8192 rows).
 PATH_KEYS = {
     'adamw',
     'add_noise',
     'add_rows|bf16',
     'attn_reg_grad',
+    'attn_reg_group|L=1',                          # product
     'attn_reg_group|L=1|full',
     'attn_reg_group|L=3|full',
+    'attn_reg_group|L=5',                          # product
     'attn_reg_total',
     'clip_embed',
     'cfg_step|cfg|t_out|unet_in',
@@ -57,6 +66,8 @@ PATH_KEYS = {
     'geglu_fwd',
     'gemv|nb=2',
     'gemv|nb=2|act_out',
+    'gemv|nb=8',                                   # product
+    'gemv|nb=8|act_out',                           # product
     'gn_bwd|add',
     'gn_bwd|silu',
     'gn_bwd|silu|add',
@@ -67,7 +78,12 @@ PATH_KEYS = {
     'gn|bf16|cluster|k=4|v4|silu',
     'gn|bf16|cluster|k=8|v2',
     'gn|bf16|cluster|k=8|v2|silu',
+    'gn|bf16|cluster|k=8|v4',                      # product
     'gn|bf16|cluster|k=8|v4|silu',
+    'gn|fp16|cluster|k=2|v2',                      # product
+    'gn|fp16|cluster|k=2|v2|silu',                 # product
+    'gn|fp16|cluster|k=2|v4',                      # product
+    'gn|fp16|cluster|k=2|v4|silu',                 # product
     'gn|fp16|cluster|k=4|v4',
     'gn|fp16|cluster|k=4|v4|silu',
     'gn|fp16|cluster|k=8|v2',
@@ -92,6 +108,8 @@ PATH_KEYS = {
     'ln|fp16|C=640',
     'lora_grad|R=16|global',
     'lora_grad|R=16|staged',
+    'lora_grad|R=32|staged',                       # product
+    'lora_grad|R=64|staged',                       # product
     'lora_pack',
     'masked_mse',
     'quick_gelu',
@@ -161,6 +179,14 @@ def test_sampling_loop(cuda, tmp_path):
 
 def test_clip_text_and_train(cuda):
     walks.clip_text_and_train(_audit, cuda)
+
+
+def test_train_sd15_full(cuda):
+    walks.train_sd15_full(_audit)
+
+
+def test_validation_sd15(cuda):
+    walks.validation_sd15(_audit)
 
 
 def test_coverage_table(cuda):
