@@ -3,10 +3,12 @@
 `EDLoRATrainer` keeps the reference's constructor (`EDLoRATrainer(**opt['models'])`, train_edlora.py:50), its public names
 (`init_new_concept`, `set_finetune_cfg`, `get_params_to_optimize`, `get_all_concept_token_ids`, `forward`,
 `delta_state_dict`, `load_delta_state_dict`) and its checkpoint layout ({'new_concept_embedding', 'text_encoder', 'unet'},
-keys f'{module}.lora_down.weight' / '.lora_up.weight', :371-378), and trains all THREE parameter groups of :82-139 — the
-new-concept embedding rows, the text-encoder LoRA and the UNet LoRA — in one captured CUDA graph: text encoder
-forward -> UNet forward -> masked MSE + attention regulariser -> UNet backward -> text encoder backward
-(mos_b200/train_engine.py + mos_b200/clip_train_engine.py).  The gradients land in ONE flat fp32 buffer (the payload of the
+keys f'{module}.lora_down.weight' / '.lora_up.weight', :371-378), and trains any non-empty subset of the THREE parameter
+groups of :82-139 — the new-concept embedding rows, the text-encoder LoRA and the UNet LoRA — in one captured CUDA graph:
+text encoder forward -> UNet forward -> masked MSE + attention regulariser -> UNet backward -> text encoder backward
+(mos_b200/train_engine.py + mos_b200/clip_train_engine.py).  A frozen group costs nothing: a UNet without LoRA runs plain
+GEMMs and no LoRA-gradient launch; a frozen text encoder without trained rows runs its forward only (no d(text
+embeddings), no CLIP backward); untrained concept rows are constants of the text encoder's token table.  The gradients land in ONE flat fp32 buffer (the payload of the
 step's single NCCL all-reduce); there is no autograd graph to call `.backward()` on.  `forward` takes images (encoded by
 the GPU VAE engine, :203-204) or already encoded latents.
 
@@ -26,6 +28,20 @@ from mos_b200.train_engine import UNET_WHERE, TrainEngine
 
 VANILLA_LORA_UNSUPPORTED = ('enable_edlora=False (vanilla LoRA with one embedding per concept) is not built on the GPU '
                             'path: the cross-attention kernels take layer-wise embeddings')
+
+
+FINETUNE_GROUPS = ('text_embedding', 'text_encoder', 'unet')
+
+
+def _n_layers(text_state_dict):
+    return 1 + max(int(k.split('.layers.')[1].split('.')[0]) for k in text_state_dict if '.layers.' in k)
+
+
+def _check_rank(lora_cfg):
+    rank = int(lora_cfg.get('rank', 4))
+    if not 1 <= rank <= 4:
+        raise ValueError('LoRA rank must be in 1..4 (fused epilogue)')
+    return rank, float(lora_cfg.get('alpha', 1.0))
 
 
 def _check_where(where, allowed, part):
@@ -252,25 +268,33 @@ class EDLoRATrainer:
 
     # ------------------------------------------------------------------------------------------ configuration
     def set_finetune_cfg(self, finetune_cfg):
-        """trainer_edlora.py:70-142: three parameter groups with their own learning rates."""
-        te, tx, un = finetune_cfg['text_embedding'], finetune_cfg['text_encoder'], finetune_cfg['unet']
-        if not (te.get('enable_tuning') and tx.get('enable_tuning') and tx.get('lora_cfg') and un.get('enable_tuning')
-                and un.get('lora_cfg')):
-            raise NotImplementedError('the GPU trainer trains the three groups of the shipped ED-LoRA configs together '
-                                      '(text_embedding, text_encoder LoRA, unet LoRA); use UNetLoRATrainer for the UNet '
-                                      'group alone')
-        tcfg, ucfg = dict(tx['lora_cfg']), dict(un['lora_cfg'])
-        self.text_where = _check_where(tcfg.pop('where'), CLIP_WHERE, 'text_encoder')
-        self.unet_where = _check_where(ucfg.pop('where'), UNET_WHERE, 'unet')
-        for c in (tcfg, ucfg):
-            if not 1 <= int(c.get('rank', 4)) <= 4:
-                raise ValueError('LoRA rank must be in 1..4 (fused epilogue)')
-        if 'weight_decay' in te:
+        """trainer_edlora.py:70-142: up to three parameter groups with their own learning rates.  A group trains iff its
+        `enable_tuning` is set (and, for the LoRA groups, a `lora_cfg` is given, :97 / :118); at least one must."""
+        te, tx, un = (finetune_cfg.get(k) or {} for k in FINETUNE_GROUPS)
+        self.train_emb = bool(te.get('enable_tuning'))
+        self.train_text = bool(tx.get('enable_tuning') and tx.get('lora_cfg'))
+        self.train_unet = bool(un.get('enable_tuning') and un.get('lora_cfg'))
+        if not (self.train_emb or self.train_text or self.train_unet):
+            raise ValueError('finetune_cfg enables no parameter group: set enable_tuning on text_embedding, text_encoder '
+                             '(with a lora_cfg) or unet (with a lora_cfg)')
+        self.text_where = self.unet_where = None
+        self.text_rank = self.unet_rank = 4
+        self.text_alpha = self.unet_alpha = 1.0
+        if self.train_emb and 'weight_decay' in te:
             raise NotImplementedError('a per-group weight_decay for the embeddings is not supported by the flat AdamW')
-        self.text_rank, self.text_alpha = int(tcfg.get('rank', 4)), float(tcfg.get('alpha', 1.0))
-        self.unet_rank, self.unet_alpha = int(ucfg.get('rank', 4)), float(ucfg.get('alpha', 1.0))
-        self.lrs = (float(te['lr']), float(tx['lr']), float(un['lr']))
-        self.params_to_optimize_iterator = [{'lr': self.lrs[0]}, {'lr': self.lrs[1]}, {'lr': self.lrs[2]}]
+        if self.train_text:
+            tcfg = dict(tx['lora_cfg'])
+            self.text_where = _check_where(tcfg.pop('where'), CLIP_WHERE, 'text_encoder')
+            self.text_rank, self.text_alpha = _check_rank(tcfg)
+        if self.train_unet:
+            ucfg = dict(un['lora_cfg'])
+            self.unet_where = _check_where(ucfg.pop('where'), UNET_WHERE, 'unet')
+            self.unet_rank, self.unet_alpha = _check_rank(ucfg)
+        self.groups = tuple(g for g, on in zip(FINETUNE_GROUPS, (self.train_emb, self.train_text, self.train_unet)) if on)
+        # the flat state keeps three learning-rate slots; an absent group has zero length and its slot is never read
+        self.lrs = tuple(float(c['lr']) if on else 0.0
+                         for c, on in zip((te, tx, un), (self.train_emb, self.train_text, self.train_unet)))
+        self.params_to_optimize_iterator = [{'lr': lr} for g, lr in zip(FINETUNE_GROUPS, self.lrs) if g in self.groups]
 
     def get_params_to_optimize(self):
         return self.params_to_optimize_iterator
@@ -279,18 +303,50 @@ class EDLoRATrainer:
     def _kaiming(self, rank, K):
         return (torch.rand(rank, K, generator=self._gen) * 2 - 1) / math.sqrt(K)       # edlora.py:238
 
+    def _topology(self):
+        c = self.unet.config
+        return dict(block_out=tuple(c.block_out_channels), layers=c.layers_per_block, heads=c.attention_head_dim,
+                    cross_dim=c.cross_attention_dim)
+
+    def lora_module_names(self):
+        """{'text_encoder': [...], 'unet': [...]}: the modules that carry a LoRA (trainer_edlora.py:100-133), empty for a
+        group that does not train"""
+        from mos_b200.clip_train_engine import CLIPTrainEngine
+        names = {'text_encoder': [], 'unet': []}
+        if self.train_text:
+            names['text_encoder'] = CLIPTrainEngine.module_names(_n_layers(self.text_encoder.state_dict()), self.text_where)
+        if self.train_unet:
+            probe = _NameProbe(self._topology(), self.unet_where)
+            names['unet'] = TrainEngine.lora_module_names.__get__(probe)()
+        return names
+
+    def flat_group_sizes(self):
+        """floats of the three groups of the flat training state [concept rows | text LoRA | UNet LoRA] (0 = absent);
+        the LoRA blocks keep rank-4 slots and the text encoder's GEMM pads"""
+        from mos_b200.clip_train_engine import CLIPTrainEngine
+        tsd = self.text_encoder.state_dict()
+        C = tsd['text_model.embeddings.token_embedding.weight'].shape[1]
+        n_text = 0
+        if self.train_text:
+            heads = getattr(self.text_encoder, 'hf_config', {}).get('num_attention_heads', 12)
+            n_inner = tsd['text_model.encoder.layers.0.mlp.fc1.weight'].shape[0]
+            n_text = CLIPTrainEngine.lora_param_count(_n_layers(tsd), C, heads * 80, where=self.text_where, inner=n_inner)
+        names = self.lora_module_names()
+        usd = self.unet.state_dict()
+        n_unet = sum(4 * (usd[m + '.weight'].reshape(usd[m + '.weight'].shape[0], -1).shape[1] + usd[m + '.weight'].shape[0])
+                     for m in names['unet'])
+        n_rows = len(self.get_all_concept_token_ids()) if self.train_emb else 0
+        return n_rows * C, n_text, n_unet
+
     def _build(self, batch):
+        from mos_b200.clip_engine import CLIPTextEngine
         from mos_b200.clip_train_engine import CLIPTrainEngine
         from mos_b200.dp import FlatTrainState
-        c = self.unet.config
-        topo = dict(block_out=tuple(c.block_out_channels), layers=c.layers_per_block, heads=c.attention_head_dim,
-                    cross_dim=c.cross_attention_dim)
+        topo = self._topology()
         usd = {k: v.detach() for k, v in self.unet.state_dict().items()}
         tsd = self.text_encoder.state_dict()
-        probe = _NameProbe(topo, self.unet_where)
-        unet_names = TrainEngine.lora_module_names.__get__(probe)()
-        n_layers = 1 + max(int(k.split('.layers.')[1].split('.')[0]) for k in tsd if '.layers.' in k)
-        text_names = CLIPTrainEngine.module_names(n_layers, self.text_where)
+        names = self.lora_module_names()
+        unet_names, text_names = names['unet'], names['text_encoder']
         ulora, tlora = {}, {}
         for m in unet_names:                                   # LoRALinearLayer init: down kaiming, up zeros (:238-239)
             w = usd[m + '.weight']
@@ -303,26 +359,37 @@ class EDLoRATrainer:
         ids = self.get_all_concept_token_ids()
         C = tsd['text_model.embeddings.token_embedding.weight'].shape[1]
         heads = getattr(self.text_encoder, 'hf_config', {}).get('num_attention_heads', 12)
-        n_inner = tsd['text_model.encoder.layers.0.mlp.fc1.weight'].shape[0]
-        n_text = CLIPTrainEngine.lora_param_count(n_layers, C, heads * 80, where=self.text_where, inner=n_inner)
-        n_unet = sum(4 * (usd[m + '.weight'].reshape(usd[m + '.weight'].shape[0], -1).shape[1] + usd[m + '.weight'].shape[0])
-                     for m in unet_names)
-        self.state = FlatTrainState(len(ids), C, n_text, n_unet, lrs=self.lrs, device=self.device)
+        _, n_text, n_unet = self.flat_group_sizes()
+        self.state = FlatTrainState(len(ids) if self.train_emb else 0, C, n_text, n_unet, lrs=self.lrs, device=self.device)
+        text_grad = self.train_emb or self.train_text
         H, W = self.latent_size
-        self.engine = TrainEngine(usd, batch, H, W, lora=ulora, lora_alpha=self.unet_alpha,
+        self.engine = TrainEngine(usd, batch, H, W, lora=ulora if self.train_unet else None, lora_alpha=self.unet_alpha,
                                   attn_reg_weight=self.attn_reg_weight, reg_full_identity=self.reg_full_identity,
-                                  state=self.state, state_offset=self.state.group_end[1], text_grad=True,
-                                  device=self.device, where=self.unet_where, **topo)
+                                  state=self.state, state_offset=self.state.group_end[1], text_grad=text_grad,
+                                  device=self.device, where=self.unet_where or UNET_WHERE[0], **topo)
         n_x = len(self.engine.xattn_names)
-        self.text_engine = CLIPTrainEngine(tsd, n_x * batch, lora=tlora, lora_alpha=self.text_alpha,
-                                           concept_token_ids=ids, state=self.state, emb_offset=0,
-                                           lora_offset=self.state.group_end[0], device=self.device, heads=heads,
-                                           where=self.text_where)
+        if text_grad:
+            self.text_engine = CLIPTrainEngine(tsd, n_x * batch, lora=tlora if self.train_text else None,
+                                               lora_alpha=self.text_alpha, concept_token_ids=ids, state=self.state,
+                                               emb_offset=0 if self.train_emb else None,
+                                               lora_offset=self.state.group_end[0], device=self.device, heads=heads,
+                                               where=self.text_where or CLIP_WHERE[0])
+        else:                       # UNet only: the text encoder (concept rows included) is a constant forward
+            self.text_engine = CLIPTextEngine(tsd, n_x * batch, device=self.device, heads=heads)
+        self._rows_dev = torch.tensor(ids, dtype=torch.long, device=self.device)
+        if not self.train_emb and ids:
+            self.state.set_const_rows(self._concept_rows())
         self.engine.attach_text_engine(self.text_engine)
         self._batch = batch
         if self._loaded is not None:
             self._apply_delta(self._loaded)
             self._loaded = None
+
+    def _concept_rows(self):
+        """the current new-concept rows fp32 [R, 768] on the device (trained, or constants of the token table)"""
+        if self.train_emb:
+            return self.text_engine.emb_view
+        return self.text_engine.tok[self._rows_dev]
 
     # ------------------------------------------------------------------------------------------ step
     def tokenize_layerwise(self, prompts):
@@ -381,23 +448,26 @@ class EDLoRATrainer:
     __call__ = forward
 
     def refresh(self):
-        """after an optimiser step on the flat state: re-pack both LoRA sets and write the embedding rows back"""
+        """after an optimiser step on the flat state: re-pack the LoRA sets and write the embedding rows back (a frozen
+        group issues nothing)"""
         self.engine.refresh_lora()
-        self.text_engine.refresh_lora()
+        if self.train_emb or self.train_text:
+            self.text_engine.refresh_lora()
 
     # ------------------------------------------------------------------------------------------ checkpoints
     def delta_state_dict(self):
-        """trainer_edlora.py:358-378."""
+        """trainer_edlora.py:358-378: the concept rows always (trained or not), the LoRAs of the groups that train (an
+        absent group leaves its section empty)."""
         if self.engine is None:
             raise RuntimeError('delta_state_dict before the first forward: the engines are built on the first batch')
         delta = {'new_concept_embedding': {}, 'text_encoder': {}, 'unet': {}}
-        rows = self.text_engine.emb_view.detach().cpu()
+        rows = self._concept_rows().detach().cpu()
         k = 0
         for concept_name, cfg in self.new_concept_cfg.items():
             n = len(cfg['concept_token_ids'])
             delta['new_concept_embedding'][concept_name] = rows[k:k + n].clone()
             k += n
-        for key, v in self.text_engine.lora_state_dict().items():
+        for key, v in (self.text_engine.lora_state_dict() if self.train_text else {}).items():
             v = v.cpu()
             delta['text_encoder'][key] = (v[:self.text_rank] if key.endswith('lora_down.weight') else v[:, :self.text_rank]).clone()
         for key, v in self.engine.lora_state_dict().items():
@@ -406,7 +476,9 @@ class EDLoRATrainer:
         return delta
 
     def load_delta_state_dict(self, delta_state_dict):
-        """trainer_edlora.py:315-356 (applied when the engines exist, i.e. at the first batch at the latest)."""
+        """trainer_edlora.py:315-356 (applied when the engines exist, i.e. at the first batch at the latest).  Unlike the
+        reference, which skips the LoRA tensors of a group it does not train (no parameter name matches them), a checkpoint
+        carrying a LoRA for such a group is refused with ValueError rather than silently half-loaded."""
         if self.engine is None:
             self._loaded = delta_state_dict
         else:
@@ -415,15 +487,23 @@ class EDLoRATrainer:
     def _apply_delta(self, delta):
         emb = delta.get('new_concept_embedding') or {}
         if emb:
+            rows = self._concept_rows().clone()
             k = 0
             for concept_name, cfg in self.new_concept_cfg.items():
                 n = len(cfg['concept_token_ids'])
                 if concept_name in emb:
-                    self.text_engine.emb_view[k:k + n].copy_(emb[concept_name].to(self.device, torch.float32))
+                    rows[k:k + n] = emb[concept_name].to(self.device, torch.float32)
                 k += n
-        if delta.get('text_encoder'):
-            self.text_engine.load_lora_state_dict(delta['text_encoder'])
-        unet = delta.get('unet') or {}
-        if unet:
-            self.engine.load_lora_state_dict(unet)
+            if self.train_emb:
+                self.text_engine.emb_view.copy_(rows)
+            else:                   # constants of the text encoder (and of the Norm_mean state)
+                self.text_engine.tok.index_copy_(0, self._rows_dev, rows)
+                if self.state.const_rows is not None:
+                    self.state.set_const_rows(rows)
+        for part, on, eng in (('text_encoder', self.train_text, self.text_engine), ('unet', self.train_unet, self.engine)):
+            if not delta.get(part):
+                continue
+            if not on:
+                raise ValueError(f'the checkpoint has a {part} LoRA but finetune_cfg does not train that group')
+            eng.load_lora_state_dict(delta[part])
         self.refresh()

@@ -194,14 +194,26 @@ class CLIPTextEngine:
         ops.gemm(A, ent['W'], out, M=M, bias=ent['bias'], residual=residual, heads=heads, lda=lda, **kw)
         self.launches += 1
 
+    def set_ids(self, input_ids):
+        """input_ids: integer [n_seq, 77] -> the static id buffer `encode` (and the training engine's forward / backward)
+        reads, so that those calls only enqueue kernels and can be captured in a CUDA graph."""
+        assert tuple(input_ids.shape) == (self.n_seq, self.T), \
+            f'expected ids of shape {(self.n_seq, self.T)}, got {tuple(input_ids.shape)}'
+        self.buf('ids', (self.n_seq * self.T,), torch.int32).copy_(input_ids.reshape(-1).to(self.dev, torch.int32))
+
     def forward(self, input_ids):
         """input_ids: integer tensor [n_seq, 77] -> last_hidden_state fp32 [n_seq, 77, 768] (after final_layer_norm)."""
+        self.set_ids(input_ids)
+        y = self.encode(self.buf('y', (self.n_seq * self.T, self.C)))
+        return y.float().view(self.n_seq, self.T, self.C)
+
+    def encode(self, out):
+        """last_hidden_state of the ids set by `set_ids` as bf16 rows [n_seq * 77, 768] of pitch out.stride(0) (e.g. a
+        training engine's in_ehs); saves nothing for a backward pass and only enqueues kernels."""
         n, T, C, Cp, Ca, Hh, dh = self.n_seq, self.T, self.C, self.Cp, self.Ca, self.heads, self.dh
-        assert tuple(input_ids.shape) == (n, T), f'expected ids of shape {(n, T)}, got {tuple(input_ids.shape)}'
         M = n * T
         self.launches = 0
         ids = self.buf('ids', (M,), torch.int32)
-        ids.copy_(input_ids.reshape(-1).to(self.dev, torch.int32))
         x = self.buf('x0', (M, Cp))
         ops.clip_embed(ids, self.tok, self.pos, x, T=T, C=C)
         self.launches += 1
@@ -237,9 +249,8 @@ class CLIPTextEngine:
             self._gemm(h, ent['fc2'], x2, M=M, residual=x1)
             x = x2
             self.launches += 4
-        y = self.buf('y', (M, C))
-        ops.layernorm(x, self.final_ln[0], self.final_ln[1], y, M=M, C=C, eps=self.eps, ldx=Cp, ldy=C)
+        ops.layernorm(x, self.final_ln[0], self.final_ln[1], out, M=M, C=C, eps=self.eps, ldx=Cp, ldy=out.stride(0))
         self.launches += 1
-        return y.float().view(n, T, C)
+        return out
 
     __call__ = forward

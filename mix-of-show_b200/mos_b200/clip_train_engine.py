@@ -15,6 +15,11 @@ gradient: no gather / scatter between the two engines.
 
 With `where: CLIPEncoderLayer` (trainer_edlora.py:100-112) mlp.fc1 / mlp.fc2 of every layer are trained too.
 
+Either group may be frozen on its own (the `enable_tuning` flags of trainer_edlora.py:82-118): with `lora=None` the GEMMs
+run plain epilogues and the backward issues no LoRA-gradient launch (it still runs through the frozen layers down to the
+embedding rows); with `emb_offset=None` the concept rows are constants of the engine's own token table and the
+embedding-row gradient launch is skipped.
+
 Flat parameter layout of a LoRA (padded to the GEMM shapes of clip_engine.py; pads are zero and stay zero: their gradients
 are exactly zero, so AdamW never moves them):
     q / k / v : down [4, 768], up [960, 4]   (12 heads of 64 dims run as 80: rows h*80+64 .. h*80+79 are pads)
@@ -37,27 +42,30 @@ class CLIPTrainEngine(CLIPTextEngine):
     def __init__(self, state_dict, n_seq, *, lora, lora_alpha=1.0, concept_token_ids=(), state=None, emb_offset=0,
                  lora_offset=None, where='CLIPAttention', **kw):
         """lora: {f'{module}.lora_down.weight' [r,768], f'{module}.lora_up.weight' [768,r]} for every q/k/v/out_proj of
-        every layer (rank <= 4).  concept_token_ids: rows of the token-embedding table that are trained.
+        every layer (rank <= 4); None = no LoRA (the text-encoder group is frozen).  concept_token_ids: the new-concept
+        rows of the token-embedding table.
         state: dp.FlatTrainState to live in (parameters / gradients are views of it): the embedding rows at
-        `emb_offset`, the LoRA block at `lora_offset`; None = a private state.
+        `emb_offset` (None = the rows are not trained and stay in the token table), the LoRA block at `lora_offset`;
+        None = a private state.
         where: the LoRA placement (CLIP_WHERE); `lora` must hold a pair for every module of lora_module_names()."""
         if where not in CLIP_WHERE:
             raise ValueError(f'where: {where!r} is not one of {CLIP_WHERE}')
         self.where = where
         super().__init__(state_dict, n_seq, lora=lora, lora_alpha=lora_alpha, **kw)
-        assert self.lora is not None, 'training needs an un-merged LoRA'
         self.concept_ids = [int(i) for i in concept_token_ids]
         R, C = len(self.concept_ids), self.C
-        n_lora = self.lora_param_count(self.n_layers, C, self.Ca, where=where, inner=self.I)
+        n_lora = self.lora_param_count(self.n_layers, C, self.Ca, where=where, inner=self.I) if lora is not None else 0
         if state is None:
             from .dp import FlatTrainState
             state = FlatTrainState(R, C, n_lora, 0, device=self.dev)
             emb_offset, lora_offset = 0, R * C
         self.state = state
-        self.emb_view = state.params[emb_offset:emb_offset + R * C].view(R, C)
-        self.emb_grad = state.grads[emb_offset:emb_offset + R * C].view(R, C)
         self.rows_dev = torch.tensor(self.concept_ids, dtype=torch.int32, device=self.dev)
-        if R:
+        self.train_rows = emb_offset is not None and R > 0
+        self.emb_view = self.emb_grad = None
+        if self.train_rows:
+            self.emb_view = state.params[emb_offset:emb_offset + R * C].view(R, C)
+            self.emb_grad = state.grads[emb_offset:emb_offset + R * C].view(R, C)
             self.emb_view.copy_(self.tok[self.rows_dev.long()])
         self._accumulate = False
         self.wb = {}
@@ -109,7 +117,7 @@ class CLIPTrainEngine(CLIPTextEngine):
         C, Ca, Cp = self.C, self.Ca, self.Cp
         self.lora_views = {}
         rows, keep = [], []
-        for m in self.lora_module_names():
+        for m in (self.lora_module_names() if lora is not None else ()):
             kd = f'{m}.lora_down.weight'
             if kd not in lora:
                 raise ValueError(f'training needs a LoRA pair on every module of `where: {self.where}`; missing {kd}')
@@ -151,7 +159,8 @@ class CLIPTrainEngine(CLIPTextEngine):
         self._lora_end = off
         self._keep = keep
         self.lora_table = torch.tensor(rows, dtype=torch.int64, device=self.dev)
-        self.load_lora_state_dict(lora)
+        if lora is not None:
+            self.load_lora_state_dict(lora)
 
     def load_lora_state_dict(self, lora):
         """reference checkpoint tensors ([r, 768] / [768, r], trainer_edlora.py:371-378) -> padded flat layout."""
@@ -201,9 +210,10 @@ class CLIPTrainEngine(CLIPTextEngine):
 
     def refresh_lora(self):
         """Re-pack the flat LoRA parameters into the forward / backward GEMM operand layouts and write the trained embedding
-        rows back into the token table (after load / optimiser step)."""
-        ops.lora_pack(self.lora_table, self.lora_table.shape[0], self.alpha)
-        if self.rows_dev.numel():
+        rows back into the token table (after load / optimiser step); a frozen group issues nothing."""
+        if self.lora_views:
+            ops.lora_pack(self.lora_table, self.lora_table.shape[0], self.alpha)
+        if self.train_rows:
             self.tok.index_copy_(0, self.rows_dev.long(), self.emb_view)
 
     # ------------------------------------------------------------------------------------------ backward packs
@@ -216,9 +226,9 @@ class CLIPTrainEngine(CLIPTextEngine):
             for s_, pj in enumerate(PROJ[:3]):
                 Wt = torch.zeros(Cp, Ca, device=self.dev, dtype=BF16)
                 Wt[:C] = Wqkv[s_ * Ca:(s_ + 1) * Ca].t()
-                self.wb[L + 'self_attn.' + pj].update(W=Wt.contiguous(), bias=None, N=Cp, K=Ca)
+                self.wb.setdefault(L + 'self_attn.' + pj, {}).update(W=Wt.contiguous(), bias=None, N=Cp, K=Ca)
             Wo = ent['out']['W']                                     # [Cp, Ca]
-            self.wb[L + 'self_attn.out_proj'].update(W=Wo[:C].t().contiguous(), bias=None, N=Ca, K=C)   # [Ca, C]
+            self.wb.setdefault(L + 'self_attn.out_proj', {}).update(W=Wo[:C].t().contiguous(), bias=None, N=Ca, K=C)
             W1 = ent['fc1']['W']                                     # [Ip, C]
             Wt = torch.zeros(Cp, self.Ip, device=self.dev, dtype=BF16)
             Wt[:C] = W1.t()
@@ -241,6 +251,8 @@ class CLIPTrainEngine(CLIPTextEngine):
         return self._lg_buf
 
     def _lora_grad(self, m, x, dy, M, ldx=None, lddy=None):
+        if not self.lora_views:
+            return                  # frozen text encoder: no LoRA gradient
         D, U, gD, gU, K, N = self.lora_views[m]
         ops.lora_grad(x, dy, D, U, self.alpha, self._lg_ws(K, N), gD, gU, M=M, K=K, N=N, ldx=ldx, lddy=lddy,
                       accumulate=self._accumulate)
@@ -248,12 +260,6 @@ class CLIPTrainEngine(CLIPTextEngine):
     # ------------------------------------------------------------------------------------------ forward (training)
     def tb(self, tag, shape, dtype=BF16, zero=False):
         return self.buf('T.' + tag, shape, dtype, zero)
-
-    def set_ids(self, input_ids):
-        """input_ids: integer [n_seq, 77] in LAYER-MAJOR order (sequence = layer * B + sample) -> the static id buffer the
-        (graph-capturable) forward / backward read."""
-        assert tuple(input_ids.shape) == (self.n_seq, self.T)
-        self.buf('ids', (self.n_seq * self.T,), torch.int32).copy_(input_ids.reshape(-1).to(self.dev, torch.int32))
 
     def forward_train(self, input_ids=None, out=None):
         """Writes the last hidden state as bf16 [n_seq * 77, 768] into `out` (e.g. the UNet engine's in_ehs) and keeps
@@ -310,7 +316,8 @@ class CLIPTrainEngine(CLIPTextEngine):
     # ------------------------------------------------------------------------------------------ backward
     def backward(self, d_y, accumulate=False):
         """d_y: bf16 [n_seq * 77, ld >= 768] = d loss / d last_hidden_state (layer-major sequence order).  Accumulates the
-        embedding-row and LoRA gradients into the flat state (`accumulate`: add to what is there)."""
+        embedding-row and LoRA gradients into the flat state (`accumulate`: add to what is there).  Returns d(embedding
+        output) [M, 800], or None with constant concept rows (the gradient of layer 0's input is then not formed)."""
         n, T, C, Cp, Ca, Hh, dh = self.n_seq, self.T, self.C, self.Cp, self.Ca, self.heads, self.dh
         M = n * T
         BH = n * Hh
@@ -325,7 +332,7 @@ class CLIPTrainEngine(CLIPTextEngine):
             ent = self.w[i]
             L = f'{self.pre}encoder.layers.{i}.'
             # ---- MLP: x2 = x1 + fc2(quick_gelu(fc1(LN2(x1))))
-            mlp_lora = self.where == 'CLIPEncoderLayer'
+            mlp_lora = self.where == 'CLIPEncoderLayer' and bool(self.lora_views)
             if mlp_lora:        # fc2's input, quick_gelu(hpre), is recomputed instead of kept
                 h = self.buf('h', (M, self.Ip))
                 ops.quick_gelu_fwd(S['hpre'], h, M=M, C=self.Ip)
@@ -360,15 +367,20 @@ class CLIPTrainEngine(CLIPTextEngine):
             ops.attention_bwd(S['Q'], S['K'], S['V'], dO, Qt, Kt, dOt, S['lse'], delta, dqkv[:, :Ca], dqkv[:, Ca:2 * Ca],
                               dqkv[:, 2 * Ca:], batch=n, heads=Hh, head_dim=dh, nq=T, nk=T, scale=self.d ** -0.5,
                               lddq=3 * Ca, lddk=3 * Ca, lddv=3 * Ca, causal=True)
+            # d(input of layer 0) only feeds the embedding-row gradient: with constant rows it is not formed
+            need_dx = i > 0 or self.train_rows
             for s_, pj in enumerate(PROJ[:3]):
                 mm = L + 'self_attn.' + pj
                 sl = dqkv[:, s_ * Ca:(s_ + 1) * Ca]
                 self._lora_grad(mm, S['ln1'], sl, M, lddy=3 * Ca)
-                self._gemm_b(sl, self.wb[mm], d_ln, M=M, lda=3 * Ca, residual=d_ln if s_ > 0 else None)
-            ops.layernorm_bwd(S['x'], d_ln, ent['ln1'][0], d_x, M=M, C=C, eps=self.eps, add=d_x1, ldx=Cp, lddy=Cp,
-                              lddx=Cp, ldadd=Cp)
+                if need_dx:
+                    self._gemm_b(sl, self.wb[mm], d_ln, M=M, lda=3 * Ca, residual=d_ln if s_ > 0 else None)
+            if need_dx:
+                ops.layernorm_bwd(S['x'], d_ln, ent['ln1'][0], d_x, M=M, C=C, eps=self.eps, add=d_x1, ldx=Cp, lddy=Cp,
+                                  lddx=Cp, ldadd=Cp)
             self.launches += 20
-        if self.rows_dev.numel():
-            ops.clip_embed_bwd(self.buf('ids', (M,), torch.int32), d_x, self.rows_dev, self.emb_grad, C=C,
-                               accumulate=self._accumulate)
+        if not self.train_rows:
+            return None
+        ops.clip_embed_bwd(self.buf('ids', (M,), torch.int32), d_x, self.rows_dev, self.emb_grad, C=C,
+                           accumulate=self._accumulate)
         return d_x

@@ -9,7 +9,10 @@ import torch.distributed as dist
 
 
 class FlatTrainState:
-    """Flat parameter / gradient / Adam-moment buffers with the three learning-rate groups of train_edlora.py:57."""
+    """Flat parameter / gradient / Adam-moment buffers with the three learning-rate groups of train_edlora.py:57.  A group
+    that does not train has zero length.  `const_rows`: when the embedding group does not train, a state of its own
+    over the (constant) concept rows, so that optimizer_step still reduces their Norm_mean every step
+    (train_edlora.py:138-140)."""
 
     def __init__(self, n_emb_rows, emb_dim, n_text_lora, n_unet_lora, lrs=(1e-3, 1e-5, 1e-4), device='cpu'):
         self.emb_rows, self.emb_dim = n_emb_rows, emb_dim
@@ -22,6 +25,23 @@ class FlatTrainState:
         self.exp_avg = torch.zeros(n, device=device)
         self.exp_avg_sq = torch.zeros(n, device=device)
         self.step = 0
+        self.const_rows = None
+
+    @property
+    def group_sizes(self):
+        return (self.group_end[0], self.group_end[1] - self.group_end[0], self.group_end[2] - self.group_end[1])
+
+    @property
+    def has_rows(self):
+        """whether optimizer_step can report Norm_mean of the concept rows"""
+        return self.emb_rows > 0 or self.const_rows is not None
+
+    def set_const_rows(self, rows):
+        """rows fp32 [R, C]: the concept rows of an untrained embedding group (see the class docstring)"""
+        R, C = rows.shape
+        c = FlatTrainState(R, C, 0, 0, lrs=(0.0, 0.0, 0.0), device=self.params.device)
+        c.params.copy_(rows.reshape(-1))
+        self.const_rows = c
 
     @property
     def n(self):
@@ -67,3 +87,9 @@ def optimizer_step(state, grad_scale, norm_out=None):
     ops.flat_adamw_step(state.params, state.grads, state.exp_avg, state.exp_avg_sq, state.group_end, state.lrs,
                         step=state.step, grad_scale=grad_scale, emb_rows=state.emb_rows, emb_dim=state.emb_dim,
                         norm_mean_out=norm_out)
+    c = state.const_rows
+    if norm_out is not None and state.emb_rows == 0 and c is not None:
+        # Norm_mean of constant rows through the same reduction: an AdamW step at learning rate 0 on zero gradients
+        # leaves the rows (and the zero moments) bit-identical: p (1 - 0 wd) - 0 m / (sqrt(v) + eps) = p
+        ops.flat_adamw_step(c.params, c.grads, c.exp_avg, c.exp_avg_sq, c.group_end, c.lrs, step=1,
+                            emb_rows=c.emb_rows, emb_dim=c.emb_dim, norm_mean_out=norm_out)

@@ -12,8 +12,11 @@ every transformer block.  The GEGLU projection's LoRA up lives in the flat state
 natural order.  The attention regulariser (cal_attn_reg, :263-313) only
 ever reads two key columns of the cross-attention maps, so the forward emits exactly those columns.
 
-VAE encoding and the CLIP text encoder (and with it the gradient w.r.t. the text embeddings) are §8f "next": this engine
-takes latents and layer-wise text embeddings as inputs.
+With `lora=None` the UNet is frozen (only text-side groups train): the forward runs plain GEMM epilogues and the backward
+runs the full dX chain down to d(text embeddings) with no LoRA-gradient or LoRA-pack launch and no LoRA rows in the
+backward packs.  The text encoder is attached with `attach_text_engine`: a training CLIPTrainEngine (text_grad=True) or a
+frozen CLIPTextEngine whose forward runs inside the same captured step (text_grad=False: no d(text embeddings) and no text
+K / V dX GEMMs).
 """
 import math
 
@@ -37,7 +40,8 @@ def _key(t):
 class TrainEngine(UNetEngine):
     def __init__(self, state_dict, batch, height, width, *, lora, lora_alpha=1.0, attn_reg_weight=0.01,
                  reg_full_identity=True, lr=1e-4, state=None, state_offset=0, text_grad=False, where='Attention', **kw):
-        """where: the LoRA placement (UNET_WHERE); `lora` must hold a pair for every module of lora_module_names().
+        """where: the LoRA placement (UNET_WHERE); `lora` must hold a pair for every module of lora_module_names(), or be
+        None for a frozen UNet (only with a shared `state`: the text encoder trains).
         state / state_offset: a shared dp.FlatTrainState (and the offset of the UNet-LoRA block in it) when the text
         encoder is trained in the same step (clip_train_engine.CLIPTrainEngine); None = a private state.
         text_grad: also produce d loss / d(text embeddings) into `self.d_ehs` (bf16 [16 * B * 77, 800], layer-major rows =
@@ -123,7 +127,9 @@ class TrainEngine(UNetEngine):
         return m if ('.attn1.' in m or '.attn2.' in m) else self._fwd_slot(m)[0]
 
     def _build_lora_state(self, lora, lr):
-        mods = self.lora_module_names()
+        mods = self.lora_module_names() if lora is not None else []
+        if lora is None and self._ext_state is None:
+            raise ValueError('a frozen UNet (lora=None) trains nothing of its own: pass the shared state of the text encoder')
         sizes = []
         for m in mods:
             kd = f'{m}.lora_down.weight'
@@ -156,7 +162,7 @@ class TrainEngine(UNetEngine):
             fdown = ent['lora_down'].data_ptr() + 4 * seg * K * 2
             fup = ent['lora_up'].data_ptr() + row_off * 4 * 4
             bdown = bup = 0
-            is_kv = m.endswith('attn2.to_k') or m.endswith('attn2.to_v')
+            is_kv = self._is_text_kv(m)
             if not is_kv or self.text_grad:
                 # text K / V projections: their input gradient d(ehs) is only needed when the text encoder trains; its
                 # width 768 is padded to the GEMM's 160-column tiles (800, zero rows)
@@ -170,11 +176,25 @@ class TrainEngine(UNetEngine):
             rows.append([D.data_ptr(), U.data_ptr(), K, N, fdown, fup, bdown, bup])
         self._lora_keep = keep
         self.lora_table = torch.tensor(rows, dtype=torch.int64, device=self.dev)
-        self.load_lora_state_dict(lora)
+        if lora is not None:
+            self.load_lora_state_dict(lora)
+
+    def _is_text_kv(self, m):
+        return m.endswith('attn2.to_k') or m.endswith('attn2.to_v')
+
+    def _frozen_bwd_entry(self, m):
+        """dX pack entry of an attention projection of a frozen UNet: no LoRA term (W is filled by _build_backward_packs)"""
+        key, _ = self._fwd_slot(m)
+        ent = self.w[key]
+        N = ent['N'] // (3 if key.endswith('.qkv') else 2 if key.endswith('.kv') else 1)
+        K = ent['K']
+        return {'N': _r(K, 160) if self._is_text_kv(m) else K, 'K': N, 'bias': None}
 
     def refresh_lora(self):
-        """Re-pack the flat LoRA parameters into the GEMM operand layouts (after load / optimiser step)."""
-        ops.lora_pack(self.lora_table, self.lora_table.shape[0], self.lora_alpha)
+        """Re-pack the flat LoRA parameters into the GEMM operand layouts (after load / optimiser step); nothing for a
+        frozen UNet."""
+        if self.lora_views:
+            ops.lora_pack(self.lora_table, self.lora_table.shape[0], self.lora_alpha)
 
     def _up_perm(self, m):
         """row permutation natural -> flat of module m's LoRA up (None = identity): the GEGLU projection's flat up is in the
@@ -242,10 +262,12 @@ class TrainEngine(UNetEngine):
         for m in self.lora_module_names():
             bk = self._bwd_key(m)
             if bk not in self.wb:
-                continue
+                if self.lora_views or (self._is_text_kv(m) and not self.text_grad):
+                    continue
+                self.wb[bk] = self._frozen_bwd_entry(m)
             key, seg = self._fwd_slot(m)
             W = self.w[key]['W']
-            N = self.lora_views[m][5]
+            N = self.wb[bk]['K']
             Wt = W[seg * N:(seg + 1) * N].t()
             if self.wb[bk]['N'] != Wt.shape[0]:                # padded output width (text K / V: 768 -> 800)
                 Wp = torch.zeros(self.wb[bk]['N'], N, device=self.dev, dtype=W.dtype)
@@ -394,6 +416,8 @@ class TrainEngine(UNetEngine):
         return out
 
     def _lora_grad(self, m, x, dy, M, ldx=None, lddy=None):
+        if not self.lora_views:
+            return                  # frozen UNet: no LoRA gradient
         D, U, gD, gU, K, N = self.lora_views[m]
         ops.lora_grad(x, dy, D, U, self.lora_alpha, self._lg_ws(M, K, N), gD, gU, M=M, K=K, N=N, ldx=ldx, lddy=lddy,
                       accumulate=self._accumulate)
@@ -663,10 +687,12 @@ class TrainEngine(UNetEngine):
 
     # ------------------------------------------------------------------------------------------ public API
     def attach_text_engine(self, text_engine):
-        """Train the text encoder in the same (captured) step: `text_engine` (clip_train_engine.CLIPTrainEngine over
-        16 * B layer-major sequences) writes its last hidden state straight into `in_ehs` before the UNet forward and
-        consumes `d_ehs` after the UNet backward.  Needs text_grad=True."""
-        assert self.text_grad and text_engine.n_seq == len(self.xattn_names) * self.B
+        """Run the text encoder in the same (captured) step: `text_engine` (over 16 * B layer-major sequences) writes its
+        last hidden state straight into `in_ehs` before the UNet forward.  With text_grad=True it is a
+        clip_train_engine.CLIPTrainEngine that consumes `d_ehs` after the UNet backward; with text_grad=False a frozen
+        clip_engine.CLIPTextEngine that runs its forward only."""
+        assert text_engine.n_seq == len(self.xattn_names) * self.B
+        assert not self.text_grad or hasattr(text_engine, 'backward'), "text_grad needs a training text engine"
         self.text = text_engine
         self._tgraphs = {}
 
@@ -715,12 +741,15 @@ class TrainEngine(UNetEngine):
     def _step(self):
         text = getattr(self, 'text', None)
         if text is not None:          # text encoder forward: last hidden states -> in_ehs (same layout, no copy)
-            text.forward_train(out=self.in_ehs.view(-1, self.cross_dim))
+            if self.text_grad:
+                text.forward_train(out=self.in_ehs.view(-1, self.cross_dim))
+            else:
+                text.encode(self.in_ehs.view(-1, self.cross_dim))
         ops.add_noise(self.x0, self.target, self.t_i32, self.alphas_cumprod, self.in_latents)
         self._run_train()
         self._loss()
         self._backward()
-        if text is not None:          # ... and its backward from d(in_ehs)
+        if text is not None and self.text_grad:          # ... and its backward from d(in_ehs)
             text.backward(self.d_ehs, accumulate=self._accumulate)
 
     def optimizer_step(self, grad_scale=1.0):

@@ -4,7 +4,7 @@
 One process per GPU (launch with torchrun for data parallelism), the batch sharded across ranks, ONE NCCL all-reduce per
 optimiser step on the flat fp32 gradient buffer [concept embedding rows | CLIP LoRA | UNet LoRA | loss, Norm_mean]
 (SURVEY.md 8e; the reference's DDP moves the whole 152 MB embedding gradient, train_edlora.py:70,128), fused flat AdamW with
-the three learning rates of trainer_edlora.py:82-139, linear learning-rate decay to zero (diffusers
+the learning rates of the groups trainer_edlora.py:82-139 enables, linear learning-rate decay to zero (diffusers
 get_scheduler('linear', warmup 0), train_edlora.py:85-90), the `Norm_mean >= emb_norm_threshold` embedding freeze
 (:138-143).  The reference's "restore every non-concept row after the step" (:133-136) needs no code here: only the concept
 rows are parameters of the flat state.
@@ -72,18 +72,21 @@ def train(trainer, batches, *, dataset_len, batch_size_per_gpu, gradient_accumul
                 lrs[0] = 0.0                       # frozen embedding rows (:141-143): lr 0 also switches the decay off
             state.lrs = tuple(lrs)
             grad_scale, mean_loss, _ = allreduce_flat(state, loss_value=float(loss))
-            optimizer_step(state, grad_scale / gradient_accumulation_steps, norm_out=norm_buf if state.emb_rows else None)
+            optimizer_step(state, grad_scale / gradient_accumulation_steps, norm_out=norm_buf if state.has_rows else None)
             refresh = getattr(trainer, 'refresh', None) or trainer.engine.refresh_lora
             refresh()
             micro = 0
             global_step += 1
             losses.append(mean_loss)
-            norm_mean = float(norm_buf) if state.emb_rows else None
-            if norm_mean is not None and not stop_emb_update and norm_mean >= emb_norm_threshold:
+            norm_mean = float(norm_buf) if state.has_rows else None
+            # the freeze only matters while the rows train (lr 0 on an empty group changes nothing)
+            if state.emb_rows and not stop_emb_update and norm_mean >= emb_norm_threshold:
                 stop_emb_update = True
             if print_freq and global_step % print_freq == 0:
+                # lr_scheduler.get_last_lr(): the groups present, in the order embedding -> text LoRA -> UNet LoRA
+                lr = ','.join(f'{x:.3e}' for x, n in zip(state.lrs, state.group_sizes) if n)
                 extra = '' if norm_mean is None else f' Norm_mean {norm_mean:.4f}'
-                log(f'iter {global_step}: loss {mean_loss:.5f} lr {state.lrs[2]:.3e}{extra}')
+                log(f'iter {global_step}: loss {mean_loss:.5f} lr {lr}{extra}')
             if save is not None and save_checkpoint_freq and global_step % save_checkpoint_freq == 0:
                 save(global_step)
         sched_k += 1
