@@ -270,13 +270,15 @@ def solve_from_gram(G, Cm, vv, n_rows, W0, iters, native=None):
 FUSION_WORKERS = int(os.environ.get('MOS_FUSION_WORKERS', '8'))
 
 
-def solve_all(jobs, iters, workers=None):
+def solve_all(jobs, iters, workers=None, to_host=True):
     """jobs: list of (name, G, Cm, vv, n_rows, W0, out_shape) - the independent per-layer problems of one fusion stage
     (gradient_fusion.py solves them one after the other, :394-455 / :518-563 / :690-745).  One L-BFGS solve is a chain of
     small kernels with a handful of host decisions per iteration and leaves the GPU mostly idle, so `workers` host threads
     drive `workers` solves at a time, each on its own CUDA stream.  Every solve runs exactly the arithmetic of the
-    sequential code (results are bit-identical whatever the concurrency).  -> {name: fused weight (fp32, CPU)}."""
+    sequential code (results are bit-identical whatever the concurrency).  -> {name: fused weight (fp32, CPU; on the
+    solving device with to_host=False)}."""
     workers = FUSION_WORKERS if workers is None else workers
+    host = (lambda t: t.cpu()) if to_host else (lambda t: t)
     if not jobs:
         return {}
     dev = jobs[0][1].device
@@ -289,11 +291,11 @@ def solve_all(jobs, iters, workers=None):
         for (name, *_, shape), (W0, *_), b in zip(jobs, setups, bests):
             Wn = W0.clone()
             ops.vec_axpby(Wn.view(-1), b, 1.0, 1.0)
-            out[name] = Wn.reshape(shape).cpu()
+            out[name] = host(Wn.reshape(shape))
         return out
     if workers <= 1 or len(jobs) == 1 or dev.type != 'cuda':
         for name, G, Cm, vv, n, W0, shape in jobs:
-            out[name] = solve_from_gram(G, Cm, vv, n, W0, iters).reshape(shape).cpu()
+            out[name] = host(solve_from_gram(G, Cm, vv, n, W0, iters).reshape(shape))
         return out
     import queue
     import threading
@@ -328,7 +330,7 @@ def solve_all(jobs, iters, workers=None):
     if errors:
         raise errors[0]
     torch.cuda.synchronize(dev)
-    return {job[0]: results[job[0]].cpu() for job in jobs}
+    return {job[0]: host(results[job[0]]) for job in jobs}
 
 
 def update_quasi_newton(K_target, V_target, W, iters, device='cuda'):
@@ -392,13 +394,31 @@ def _merged(W0, down, up, alpha, device):
     return Wc
 
 
+def lora_weight_names(lora_list):
+    """sorted '<module>.weight' names of every layer some LoRA of `lora_list` touches: the weights a stage solves"""
+    return sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in lora_list for k in t})
+
+
+def _owned(names, solve_names):
+    """the names this call solves (all of them for solve_names=None), in the stage's own order"""
+    if solve_names is None:
+        return names
+    own = set(solve_names)
+    return [n for n in names if n in own]
+
+
 def merge_kv_in_cross_attention(unet_state_dict, cross_kv_layer_names, text_features, unet_crosskv_list, alphas,
-                                optimize_iters, device='cuda'):
+                                optimize_iters, device='cuda', solve_names=None):
     """Cross-attention K/V fusion (gradient_fusion.py:325-457).  text_features[c][layer_idx] = CLIP features of
     concept c at its concept-token (+EOS) positions [n_pos, 768] (gradient_fusion.py:182-199; CLIP runs upstream).
-    cross_kv_layer_names: [(layer_idx, 'down_blocks....attn2.to_k.weight'), ...] in the reference's order."""
+    cross_kv_layer_names: [(layer_idx, 'down_blocks....attn2.to_k.weight'), ...] in the reference's order.
+    solve_names: solve (and return, still on the device) only these weights - one rank's share of a sharded fusion
+    (fusion_plan); every weight is bit-identical to the same weight of the full call."""
     jobs = []
+    own = None if solve_names is None else set(solve_names)
     for layer_idx, name in cross_kv_layer_names:
+        if own is not None and name not in own:
+            continue
         W0 = unet_state_dict[name].to(device, F32)
         d_in = W0.shape[1]
         G = torch.zeros(d_in, d_in, device=device)
@@ -417,7 +437,7 @@ def merge_kv_in_cross_attention(unet_state_dict, cross_kv_layer_names, text_feat
             vv += float((Wc.double() * WG.double()).sum())
             n += X.shape[0]
         jobs.append((name, G, Cm, vv, n, W0, tuple(W0.shape)))
-    return solve_all(jobs, optimize_iters)
+    return solve_all(jobs, optimize_iters, to_host=solve_names is None)
 
 
 class _RowRecorder:
@@ -461,7 +481,7 @@ def record_key(name):
 
 
 def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, optimize_iters, device='cuda',
-                       pad_id=49407):
+                       pad_id=49407, solve_names=None):
     """Text-encoder fusion (gradient_fusion.py:460-565).  text_encoder_list[c]: concept c's CLIP LoRA
     ({'text_model.encoder.layers.{i}.self_attn.{q,k,v,out}_proj.lora_{down,up}.weight'}, with `where: CLIPEncoderLayer`
     also '...layers.{i}.mlp.fc{1,2}.lora_{down,up}.weight'); prompt_ids[c]: the un-padded
@@ -470,9 +490,12 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
     the inputs of the LoRA'd linears at ALL valid token positions are recorded (the reference's forward hooks, :146-167,
     :525-541); every layer is then solved from the accumulated Gram matrices as in merge_kv_in_cross_attention.
     Causal attention makes the features of a valid position independent of the padding behind it, so the sequences are
-    padded to 77 for the engine and only the valid rows are kept."""
+    padded to 77 for the engine and only the valid rows are kept.  solve_names: as merge_kv_in_cross_attention; only
+    the inputs of these weights are recorded, and nothing runs when there are none."""
     from mos_b200.clip_engine import CLIPTextEngine
-    names = sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in text_encoder_list for k in t})
+    names = _owned(lora_weight_names(text_encoder_list), solve_names)
+    if not names:
+        return {}
     keys = {record_key(n) for n in names}
     feats = []
     for c, tuned in enumerate(text_encoder_list):
@@ -511,7 +534,7 @@ def merge_text_encoder(text_state_dict, text_encoder_list, alphas, prompt_ids, o
             vv += float((Wc.double() * WG.double()).sum())
             n += X.shape[0]
         jobs.append((name, G, Cm, vv, n, W0, tuple(W0.shape)))
-    return solve_all(jobs, optimize_iters)
+    return solve_all(jobs, optimize_iters, to_host=solve_names is None)
 
 
 class GramRecorder:
@@ -541,20 +564,23 @@ class GramRecorder:
 
 def merge_spatial_attention(unet_state_dict, unet_spatial_attn_list, alphas, concept_embeds, optimize_iters,
                             latent_hw=(64, 64), num_inference_steps=20, seed=0, device='cuda', block_out=None,
-                            layers=None):
+                            layers=None, solve_names=None):
     """Spatial-attention fusion (gradient_fusion.py:627-747).  concept_embeds[c] = layer-wise prompt embeddings
     [1,16,77,768] of 'photo of a <concept c>' (CLIP runs upstream).  For every concept: merge its LoRA, run the
     20-step DPM-Solver++ sampling (batch 1, no CFG, all steps recorded, :579-624) on the engine with the Gram
     recorder, then solve every LoRA'd layer from the accumulated Gram matrices.  Besides the attention projections this
     covers the `where: Transformer2DModel` layers (proj_in / proj_out as 1x1 convs, returned 4-D; ff.net.0.proj solved in
-    the state-dict row order, ff.net.2)."""
+    the state-dict row order, ff.net.2).  solve_names: as merge_text_encoder (every concept's sampling still runs in full
+    when some are given: the recorded inputs depend on the whole UNet)."""
     from mos_b200.engine import UNetEngine, ehs_to_layer_major
     from mos_b200.scheduler import DPMSolverPP2M
     H, Wd = latent_hw
     kw = {}
     if block_out is not None:
         kw = dict(block_out=block_out, layers=layers)
-    names = sorted({k.replace('.lora_down', '').replace('.lora_up', '') for t in unet_spatial_attn_list for k in t})
+    names = _owned(lora_weight_names(unet_spatial_attn_list), solve_names)
+    if not names:
+        return {}
     keys = {record_key(n) for n in names}
     grams, merged_w = [], []
     eng = None
@@ -616,7 +642,7 @@ def merge_spatial_attention(unet_state_dict, unet_spatial_attn_list, alphas, con
             n += grams[c].rows[rec_key]
         jobs.append((name, G, Cm, vv, n, W0, tuple(unet_state_dict[name].shape)))
     mark('solve')
-    out = solve_all(jobs, optimize_iters)
+    out = solve_all(jobs, optimize_iters, to_host=solve_names is None)
     mark('end')
     if prof:
         agg = {}
@@ -745,15 +771,66 @@ def cross_kv_layer_names(unet):
     return names
 
 
+# ------------------------------------------------------------------------------------------------ sharding across ranks
+def solve_cost(shape, iters):
+    """planned cost of one layer solve: out * in^2 * iters, the fp64 closure GEMM D G of every L-BFGS iteration
+    ([out, in] x [in, in]; a 1x1 conv [out, in, 1, 1] solves as [out, in])"""
+    out_f, in_f = shape[0], math.prod(shape[1:])
+    return out_f * in_f * in_f * iters
+
+
+def fusion_plan(shapes, iters, world):
+    """Which rank solves which weight of one fusion stage: shapes {name: weight shape} of the weights the stage solves ->
+    plan[r] = sorted names rank r owns.  Longest-processing-time-first greedy on solve_cost (ties broken by name, each
+    job to the least-loaded rank, ties to the lowest rank): the most loaded rank carries at most 4/3 of the optimum.  The
+    plan depends on names, shapes and `iters` only, so every rank computes the same one before any GPU work."""
+    load = [0] * world
+    plan = [[] for _ in range(world)]
+    for name in sorted(shapes, key=lambda n: (-solve_cost(shapes[n], iters), n)):
+        r = min(range(world), key=lambda i: (load[i], i))
+        load[r] += solve_cost(shapes[name], iters)
+        plan[r].append(name)
+    return [sorted(p_) for p_ in plan]
+
+
+def _sharded(stage, shapes, iters, rank, world, device, args, kw):
+    """Runs `stage(*args, **kw)` on this rank's share of `shapes` (fusion_plan) and exchanges the solved weights: every rank
+    returns all of them (on the host).  `device`: the device the stage runs on.  A stage that raises on any rank raises on every rank (the failing rank re-raises its own error)
+    before the exchange, so no rank is left waiting in a collective."""
+    from mos_b200 import dp
+    plan = fusion_plan(shapes, iters, world)
+    err, owned = None, {}
+    try:
+        owned = stage(*args, solve_names=plan[rank], **kw)
+    except Exception as exc:                  # reported to the other ranks first, then re-raised below
+        err = exc
+    if not dp.all_ranks_ok(err is None, device):
+        if err is not None:
+            raise err
+        raise RuntimeError(f'{stage.__name__} failed on another rank')
+    return {n: w.cpu() for n, w in dp.broadcast_owned(owned, plan, shapes, device).items()}
+
+
 def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, pretrained_model_path, save_path, suffix,
                      device='cuda', tokenizer=None, log=print):
     """gradient_fusion.py:750-813 on the GPU path.  `pretrained_model_path`: diffusers-layout directory (unet/,
     text_encoder/, tokenizer/); the fused UNet / text encoder and new_concept_cfg.json are written to
     `{save_path}/combined_model_{suffix}` together with the tokenizer that carries the added `<new{k}>` tokens (the VAE /
-    scheduler folders of the base model are untouched by the fusion and are not copied here)."""
+    scheduler folders of the base model are untouched by the fusion and are not copied here).
+    With torch.distributed initialised, the layer solves of every stage are sharded over the ranks (fusion_plan): each rank
+    replays the recording, solves its own layers and receives the others' (_sharded); the fused model is the one of a
+    single process, bit for bit.  Only rank 0 writes it, and every rank returns once it is written."""
     import os
+    import torch.distributed as dist
     from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt
     from mixofshow.utils import model_io
+    world = dist.get_world_size() if dist.is_initialized() else 1
+    rank = dist.get_rank() if world > 1 else 0
+
+    def run(stage, shapes, iters, *args, **kw):
+        if world == 1:
+            return stage(*args, **kw)
+        return _sharded(stage, shapes, iters, rank, world, device, args, kw)
     log('------Step 1: load stable diffusion checkpoint------')
     unet = model_io.load_unet(pretrained_model_path)
     text_encoder = model_io.load_text_encoder(pretrained_model_path, device=device)
@@ -776,10 +853,10 @@ def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, p
     if any(item is not None for item in text_encoder_list):
         log('------Step 4: merge text encoder------')
         ids = [[torch.tensor(_unpadded_ids(p_, tokenizer)) for p_ in prompts_of(c)] for c in concept_list]
-        new_w = merge_text_encoder(text_encoder.state_dict(), text_encoder_list,
-                                   [c['text_encoder_alpha'] for c in concept_list], ids, optimize_textenc_iters,
-                                   device=device)
         sd = text_encoder.state_dict()
+        shapes = {n: tuple(sd[n].shape) for n in lora_weight_names(text_encoder_list)}
+        new_w = run(merge_text_encoder, shapes, optimize_textenc_iters, sd, text_encoder_list,
+                    [c['text_encoder_alpha'] for c in concept_list], ids, optimize_textenc_iters, device=device)
         sd.update(new_w)
         text_encoder.load_state_dict(sd)
     if any(item is not None for item in unet_crosskv_list):
@@ -790,9 +867,11 @@ def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, p
             n = len(cp) // NUM_CROSS_ATTENTION_LAYERS
             feats.append({i: get_text_feature([cp[j * NUM_CROSS_ATTENTION_LAYERS + i] for j in range(n)], tokenizer,
                                               text_encoder, device).cpu() for i in range(NUM_CROSS_ATTENTION_LAYERS)})
-        new_w = merge_kv_in_cross_attention(unet.state_dict(), cross_kv_layer_names(unet), feats, unet_crosskv_list,
-                                            [c['unet_alpha'] for c in concept_list], optimize_textenc_iters, device=device)
         sd = unet.state_dict()
+        kv_names = cross_kv_layer_names(unet)
+        shapes = {n: tuple(sd[n].shape) for _, n in kv_names}
+        new_w = run(merge_kv_in_cross_attention, shapes, optimize_textenc_iters, sd, kv_names, feats, unet_crosskv_list,
+                    [c['unet_alpha'] for c in concept_list], optimize_textenc_iters, device=device)
         sd.update(new_w)
         unet.load_state_dict(sd)
     if any(item is not None for item in unet_spatial_attn_list):
@@ -801,15 +880,18 @@ def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, p
                                    tokenizer, text_encoder, device, return_type='full_embedding').unsqueeze(0).cpu()
                   for c in concept_list]
         cfg = unet.config
-        new_w = merge_spatial_attention(unet.state_dict(), unet_spatial_attn_list,
-                                        [c['unet_alpha'] for c in concept_list], embeds, optimize_unet_iters,
-                                        device=device, block_out=tuple(cfg.block_out_channels),
-                                        layers=cfg.layers_per_block)
         sd = unet.state_dict()
+        shapes = {n: tuple(sd[n].shape) for n in lora_weight_names(unet_spatial_attn_list)}
+        new_w = run(merge_spatial_attention, shapes, optimize_unet_iters, sd, unet_spatial_attn_list,
+                    [c['unet_alpha'] for c in concept_list], embeds, optimize_unet_iters, device=device,
+                    block_out=tuple(cfg.block_out_channels), layers=cfg.layers_per_block)
         sd.update(new_w)
         unet.load_state_dict(sd)
     out_dir = os.path.join(save_path, f'combined_model_{suffix}')
-    model_io.save_combined_model(out_dir, unet, text_encoder, new_concept_cfg, tokenizer=tokenizer)
+    if rank == 0:
+        model_io.save_combined_model(out_dir, unet, text_encoder, new_concept_cfg, tokenizer=tokenizer)
+    if world > 1:
+        dist.barrier()
     return out_dir, new_concept_cfg
 
 
@@ -825,12 +907,40 @@ def parse_args(argv=None):
     return parser.parse_args(argv)
 
 
-def main(argv=None):
-    args = parse_args(argv)
-    os.makedirs(args.save_path, exist_ok=True)
-    return compose_concepts(args.concept_cfg, args.optimize_textenc_iters, args.optimize_unet_iters, args.pretrained_models,
-                            args.save_path, args.suffix, device='cuda')
+def init_distributed():
+    """torchrun environment (WORLD_SIZE / RANK / LOCAL_RANK, as train_edlora.py reads it) -> (rank, world, device).  Ranks
+    take device LOCAL_RANK modulo the visible devices: NCCL when every rank has a GPU of its own, gloo when ranks share
+    one (more ranks on this node, LOCAL_WORLD_SIZE, than visible devices).  Without WORLD_SIZE nothing is initialised:
+    (0, 1, 'cuda')."""
+    import torch.distributed as dist
+    world = int(os.environ.get('WORLD_SIZE', '1'))
+    if world == 1:
+        return 0, 1, 'cuda'
+    n_dev = torch.cuda.device_count()
+    device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0')) % n_dev}"
+    torch.cuda.set_device(device)
+    if int(os.environ.get('LOCAL_WORLD_SIZE', world)) <= n_dev:
+        dist.init_process_group('nccl', device_id=torch.device(device))
+    else:
+        dist.init_process_group('gloo')
+    return dist.get_rank(), world, device
 
+
+def main(argv=None):
+    """`python gradient_fusion.py ...`, or under torchrun with the layer solves sharded across the ranks
+    (init_distributed, compose_concepts); only rank 0 logs."""
+    import torch.distributed as dist
+    args = parse_args(argv)
+    rank, world, device = init_distributed()
+    try:
+        if rank == 0:
+            os.makedirs(args.save_path, exist_ok=True)
+        return compose_concepts(args.concept_cfg, args.optimize_textenc_iters, args.optimize_unet_iters,
+                                args.pretrained_models, args.save_path, args.suffix, device=device,
+                                log=print if rank == 0 else (lambda *a, **k: None))
+    finally:
+        if world > 1:
+            dist.destroy_process_group()
 
 if __name__ == '__main__':
     main()

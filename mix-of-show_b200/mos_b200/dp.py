@@ -3,7 +3,11 @@ ranks, weights are replicated, and the ONLY data-path collective is a single all
 flat fp32 buffer [concept rows | text-encoder LoRA | UNet LoRA | 2 logged scalars] (4.47 MB for SD1.5), replacing the
 156 MB the reference's DDP moves (train_edlora.py:70,128; util.py:203-229).  torch.distributed is the transport
 (NCCL over NVLink on the GPU box, gloo in the CPU tests); the arithmetic after it is mos_flat_adamw_step.
+Gradient fusion shards by layer instead (gradient_fusion.fusion_plan): every rank solves its own layers and the solved
+weights are broadcast by their owners (all_ranks_ok, broadcast_owned).
 """
+import math
+
 import torch
 import torch.distributed as dist
 
@@ -76,6 +80,46 @@ def allreduce_flat_device(state, loss_dev=None, group=None):
     if world > 1:
         dist.all_reduce(state.grads, op=dist.ReduceOp.SUM, group=group)
     return 1.0 / world
+
+
+def collective_device(device):
+    """device the tensors of a collective live on: `device` under NCCL, host memory under gloo (which the ranks use when
+    they share one GPU)"""
+    return torch.device('cpu') if dist.get_backend() == 'gloo' else torch.device(device)
+
+
+def all_ranks_ok(ok, device):
+    """MIN-all-reduce of a success flag before a result exchange: a rank whose work raised says so here, so every rank
+    learns of the failure instead of waiting in a broadcast that rank never joins."""
+    flag = torch.tensor([1 if ok else 0], dtype=torch.int32, device=collective_device(device))
+    dist.all_reduce(flag, op=dist.ReduceOp.MIN)
+    return bool(flag.item())
+
+
+def broadcast_owned(owned, plan, shapes, device):
+    """Exchange of a sharded gradient-fusion stage: plan[r] lists the weights rank r solved (gradient_fusion.fusion_plan),
+    `owned` holds this rank's as fp32 tensors on `device`.  Each owner broadcasts its weights in plan order as ONE flat
+    buffer, so a stage costs `world` broadcasts whatever its layer count.  -> {name: fp32 tensor of shapes[name]} for every
+    weight of the plan: this rank's own tensors as given, the others' on collective_device(device) (host memory under
+    gloo, where the caller wants them next)."""
+    rank = dist.get_rank()
+    wire = collective_device(device)
+    out = {}
+    for r, names in enumerate(plan):
+        if not names:
+            continue
+        sizes = [math.prod(shapes[n]) for n in names]
+        if r == rank:
+            buf = torch.cat([owned[n].reshape(-1) for n in names]).to(wire, torch.float32)
+        else:
+            buf = torch.empty(sum(sizes), dtype=torch.float32, device=wire)
+        dist.broadcast(buf, src=r)
+        if r == rank:
+            out.update((n, owned[n]) for n in names)
+            continue
+        for n, part in zip(names, buf.split(sizes)):
+            out[n] = part.view(shapes[n])
+    return out
 
 
 def optimizer_step(state, grad_scale, norm_out=None):

@@ -7,6 +7,10 @@ the wall-clock seconds of every stage and the card they were measured on.
 
     python tools/compose_bench.py [--concepts 5] [--textenc-iters 500] [--unet-iters 50] [--tiny]
                                   [--unet-where {Attention,Transformer2DModel}] [--text-where {CLIPAttention,CLIPEncoderLayer}]
+
+Under `torchrun --nproc-per-node N` the layer solves are sharded over the ranks (gradient_fusion.fusion_plan); the stage
+seconds are then the maximum over the ranks, and `plan` gives every rank's layer count and share of the planned cost per
+stage.
 """
 import argparse
 import json
@@ -110,54 +114,32 @@ def main():
     ap.add_argument('--unet-where', choices=('Attention', 'Transformer2DModel'), default='Attention')
     ap.add_argument('--text-where', choices=('CLIPAttention', 'CLIPEncoderLayer'), default='CLIPAttention')
     a = ap.parse_args()
+    import torch.distributed as dist
     import gradient_fusion as gf
-    from mixofshow.models.unet_b200 import UNet2DConditionModel
-    from mixofshow.utils import model_io
-    from transformers import CLIPTextConfig, CLIPTextModel
-    work = tempfile.mkdtemp(prefix='compose_bench_')
+    from mos_b200 import dp
+    rank, world, device = gf.init_distributed()
+    plans = []
+    fusion_plan = gf.fusion_plan
+
+    def plan_and_note(shapes, iters, w):
+        plans.append((shapes, iters, fusion_plan(shapes, iters, w)))
+        return plans[-1][2]
+
+    gf.fusion_plan = plan_and_note
+    work = [tempfile.mkdtemp(prefix='compose_bench_') if rank == 0 else None]
+    if world > 1:
+        dist.broadcast_object_list(work)
+    work = work[0]
     out = {'config': f'gradient_fusion.compose_concepts, {a.concepts} synthetic ED-LoRAs, '
-                     f'{"tiny" if a.tiny else "SD1.5-size"} UNet + 12-layer CLIP text encoder, 1xH100',
-           'textenc_iters': a.textenc_iters, 'unet_iters': a.unet_iters, 'unet_where': a.unet_where,
+                     f'{"tiny" if a.tiny else "SD1.5-size"} UNet + 12-layer CLIP text encoder, {world} rank(s) on '
+                     f'{torch.cuda.device_count()} visible H100(s)',
+           'world_size': world, 'textenc_iters': a.textenc_iters, 'unet_iters': a.unet_iters, 'unet_where': a.unet_where,
            'text_where': a.text_where, 'gpu': gpu_card()}
     try:
-        t0 = time.perf_counter()
-        sd, _, _, _, cfg = bench.build_workload(a.tiny)
-        unet = UNet2DConditionModel(**(cfg or {}))
-        unet.load_state_dict(sd)
-        base = os.path.join(work, 'base')
-        model_io.save_unet(unet, base)
-        torch.manual_seed(1)
-        clip = CLIPTextModel(CLIPTextConfig(vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
-                                            num_attention_heads=12, max_position_embeddings=77, hidden_act='quick_gelu')).eval()
-        clip.save_pretrained(os.path.join(base, 'text_encoder'))
-        csd = clip.state_dict()
-        cfgs = []
-        for c in range(a.concepts):
-            g = torch.Generator().manual_seed(50 + c)
-            words = [f'<c{c}a>', f'<c{c}b>']
-            tlora = {}
-            for i in range(12):
-                for pj in ('q_proj', 'k_proj', 'v_proj', 'out_proj'):
-                    m = f'text_model.encoder.layers.{i}.self_attn.{pj}'
-                    tlora[m + '.lora_down.weight'] = (torch.rand(4, 768, generator=g) * 2 - 1) / 768 ** 0.5
-                    tlora[m + '.lora_up.weight'] = torch.randn(768, 4, generator=g) * 0.02
-            if a.text_where == 'CLIPEncoderLayer':
-                gm = torch.Generator().manual_seed(1050 + c)
-                for i in range(12):
-                    for fc in ('fc1', 'fc2'):
-                        m = f'text_model.encoder.layers.{i}.mlp.{fc}'
-                        tlora[m + '.lora_down.weight'], tlora[m + '.lora_up.weight'] = _lora_pair(gm, csd[m + '.weight'])
-            ulora = (whole_block_unet_lora(sd, cfg, seed=10 + c) if a.unet_where == 'Transformer2DModel'
-                     else bench.random_unet_lora(sd, cfg, seed=10 + c))
-            params = {'new_concept_embedding': {w: torch.randn(16, 768, generator=g) * 0.02 for w in words},
-                      'text_encoder': tlora, 'unet': ulora}
-            path = os.path.join(work, f'concept{c}.pth')
-            torch.save({'params': params}, path)
-            cfgs.append({'lora_path': path, 'unet_alpha': 1.0, 'text_encoder_alpha': 1.0, 'concept_name': ' '.join(words)})
-        cfg_path = os.path.join(work, 'concepts.json')
-        json.dump(cfgs, open(cfg_path, 'w'))
-        del unet, clip, csd
-        out['setup_seconds'] = round(time.perf_counter() - t0, 2)
+        if rank == 0:
+            write_workload(a, work, out)
+        if world > 1:
+            dist.barrier()
         stamps = []
 
         def log(msg, *rest):
@@ -165,33 +147,105 @@ def main():
             stamps.append((time.perf_counter(), str(msg)))
 
         t1 = time.perf_counter()
-        out_dir, new_cfg = gf.compose_concepts(cfg_path, a.textenc_iters, a.unet_iters, base, os.path.join(work, 'out'), 'bench',
-                                               device='cuda', tokenizer=WordTokenizer(), log=log)
+        out_dir, new_cfg = gf.compose_concepts(os.path.join(work, 'concepts.json'), a.textenc_iters, a.unet_iters,
+                                               os.path.join(work, 'base'), os.path.join(work, 'out'), 'bench',
+                                               device=device, tokenizer=WordTokenizer(), log=log)
         torch.cuda.synchronize()
         t2 = time.perf_counter()
         stamps.append((t2, 'end'))
-        stage = {}
-        for (ta, name), (tb, _) in zip(stamps[:-1], stamps[1:]):
-            key = name.strip('-')
-            stage[key] = round(tb - ta, 2)
-        out['stage_seconds'] = stage
-        out['compose_concepts_seconds'] = round(t2 - t1, 2)
+        secs = [tb - ta for (ta, _), (tb, _) in zip(stamps[:-1], stamps[1:])] + [t2 - t1]
+        if world > 1:                                   # every rank logged the same stages: slowest rank per stage
+            t = torch.tensor(secs, dtype=torch.float64, device=dp.collective_device(device))
+            dist.all_reduce(t, op=dist.ReduceOp.MAX)
+            secs = t.tolist()
+        out['stage_seconds'] = {name.strip('-'): round(v, 2) for (_, name), v in zip(stamps[:-1], secs)}
+        out['compose_concepts_seconds'] = round(secs[-1], 2)
+        if world > 1:
+            stages = ('text_encoder', 'cross_kv', 'spatial')
+            out['plan'] = {}
+            for stage, (shapes, iters, plan) in zip(stages, plans):
+                cost = [sum(gf.solve_cost(shapes[n], iters) for n in p) for p in plan]
+                out['plan'][stage] = {'layers': [len(p) for p in plan],
+                                      'cost_share': [round(c / max(1, sum(cost)), 4) for c in cost]}
         out['new_concept_tokens'] = sum(len(v['concept_token_ids']) for v in new_cfg.values())
-        # the fused directory must load again (from_pretrained layout) and carry finite weights
-        fused = model_io.load_unet(out_dir)
-        w = fused.state_dict()['down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight']
-        out['fused_reload_ok'] = bool(torch.isfinite(w).all())
-        d0 = sd['down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight']
-        out['example_crosskv_delta_rel'] = round(((w.float().cpu() - d0).norm() / d0.norm()).item(), 5)
-        if a.unet_where == 'Transformer2DModel':
-            k = 'mid_block.attentions.0.transformer_blocks.0.ff.net.2.weight'
-            w = fused.state_dict()[k].float().cpu()
-            out['example_ff2_delta_rel'] = round(((w - sd[k]).norm() / sd[k].norm()).item(), 5)
-            out['fused_reload_ok'] = out['fused_reload_ok'] and bool(torch.isfinite(w).all())
-        out['data'] = 'synthetic (random-init weights, random LoRAs up ~ N(0, 0.02^2), whitespace tokenizer stub)'
+        if rank == 0:
+            check_fused(a, out_dir, out)
     finally:
-        shutil.rmtree(work, ignore_errors=True)
-    print(json.dumps(out))
+        if world > 1:
+            dist.barrier()
+            dist.destroy_process_group()
+        if rank == 0:
+            shutil.rmtree(work, ignore_errors=True)
+    if rank == 0:
+        print(json.dumps(out))
+
+
+def write_workload(a, work, out):
+    """the synthetic base model directory, the concept checkpoints and concepts.json under `work`"""
+    from mixofshow.models.unet_b200 import UNet2DConditionModel
+    from mixofshow.utils import model_io
+    from transformers import CLIPTextConfig, CLIPTextModel
+    t0 = time.perf_counter()
+    sd, _, _, _, cfg = bench.build_workload(a.tiny)
+    unet = UNet2DConditionModel(**(cfg or {}))
+    unet.load_state_dict(sd)
+    base = os.path.join(work, 'base')
+    model_io.save_unet(unet, base)
+    torch.manual_seed(1)
+    clip = CLIPTextModel(CLIPTextConfig(vocab_size=49408, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
+                                        num_attention_heads=12, max_position_embeddings=77, hidden_act='quick_gelu')).eval()
+    clip.save_pretrained(os.path.join(base, 'text_encoder'))
+    csd = clip.state_dict()
+    cfgs = []
+    for c in range(a.concepts):
+        g = torch.Generator().manual_seed(50 + c)
+        words = [f'<c{c}a>', f'<c{c}b>']
+        tlora = {}
+        for i in range(12):
+            for pj in ('q_proj', 'k_proj', 'v_proj', 'out_proj'):
+                m = f'text_model.encoder.layers.{i}.self_attn.{pj}'
+                tlora[m + '.lora_down.weight'] = (torch.rand(4, 768, generator=g) * 2 - 1) / 768 ** 0.5
+                tlora[m + '.lora_up.weight'] = torch.randn(768, 4, generator=g) * 0.02
+        if a.text_where == 'CLIPEncoderLayer':
+            gm = torch.Generator().manual_seed(1050 + c)
+            for i in range(12):
+                for fc in ('fc1', 'fc2'):
+                    m = f'text_model.encoder.layers.{i}.mlp.{fc}'
+                    tlora[m + '.lora_down.weight'], tlora[m + '.lora_up.weight'] = _lora_pair(gm, csd[m + '.weight'])
+        ulora = (whole_block_unet_lora(sd, cfg, seed=10 + c) if a.unet_where == 'Transformer2DModel'
+                 else bench.random_unet_lora(sd, cfg, seed=10 + c))
+        params = {'new_concept_embedding': {w: torch.randn(16, 768, generator=g) * 0.02 for w in words},
+                  'text_encoder': tlora, 'unet': ulora}
+        path = os.path.join(work, f'concept{c}.pth')
+        torch.save({'params': params}, path)
+        cfgs.append({'lora_path': path, 'unet_alpha': 1.0, 'text_encoder_alpha': 1.0, 'concept_name': ' '.join(words)})
+    cfg_path = os.path.join(work, 'concepts.json')
+    json.dump(cfgs, open(cfg_path, 'w'))
+    del unet, clip, csd
+    out['setup_seconds'] = round(time.perf_counter() - t0, 2)
+
+
+def check_fused(a, out_dir, out):
+    """the fused directory must load again (from_pretrained layout) and carry finite weights"""
+    import hashlib
+    from mixofshow.utils import model_io
+    sd, _, _, _, _ = bench.build_workload(a.tiny)
+    fused = model_io.load_unet(out_dir)
+    h = hashlib.sha256()
+    for k, v in sorted(fused.state_dict().items()):
+        h.update(k.encode())
+        h.update(v.detach().float().contiguous().numpy().tobytes())
+    out['fused_unet_sha256'] = h.hexdigest()[:16]
+    w = fused.state_dict()['down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight']
+    out['fused_reload_ok'] = bool(torch.isfinite(w).all())
+    d0 = sd['down_blocks.0.attentions.0.transformer_blocks.0.attn2.to_k.weight']
+    out['example_crosskv_delta_rel'] = round(((w.float().cpu() - d0).norm() / d0.norm()).item(), 5)
+    if a.unet_where == 'Transformer2DModel':
+        k = 'mid_block.attentions.0.transformer_blocks.0.ff.net.2.weight'
+        w = fused.state_dict()[k].float().cpu()
+        out['example_ff2_delta_rel'] = round(((w - sd[k]).norm() / sd[k].norm()).item(), 5)
+        out['fused_reload_ok'] = out['fused_reload_ok'] and bool(torch.isfinite(w).all())
+    out['data'] = 'synthetic (random-init weights, random LoRAs up ~ N(0, 0.02^2), whitespace tokenizer stub)'
 
 
 if __name__ == '__main__':
