@@ -44,6 +44,23 @@ def _check_rank(lora_cfg):
     return rank, float(lora_cfg.get('alpha', 1.0))
 
 
+def check_lora_ranks(lora, rank, part):
+    """Refuses (ValueError) a LoRA state dict of `part` ('unet' / 'text_encoder') whose rank is not the configured `rank`:
+    every lora_down [r, K] (or [r, K, 1, 1]) and lora_up [N, r] (or [N, r, 1, 1]) must have r == rank, and a module's down
+    and up must agree.  The flat training state keeps four rank slots per module whatever the rank, so a mismatch would
+    otherwise load without error: a rank-4 checkpoint under `rank: 2` trains four ranks and saves two, a rank-2 checkpoint
+    under `rank: 4` trains two and saves two zero rows.  The reference raises here too: it copies each tensor into a
+    parameter of the configured shape (trainer_edlora.py:335-340)."""
+    modules = dict.fromkeys(k.rsplit('.lora_', 1)[0] for k in lora if k.endswith(('.lora_down.weight', '.lora_up.weight')))
+    for m in modules:
+        d, u = lora.get(m + '.lora_down.weight'), lora.get(m + '.lora_up.weight')
+        ranks = {r for r in (d.shape[0] if d is not None else None, u.shape[1] if u is not None else None) if r is not None}
+        if ranks != {rank}:
+            shapes = ', '.join(f'lora_{s} {tuple(t.shape)}' for s, t in (('down', d), ('up', u)) if t is not None)
+            why = 'down and up disagree on the rank' if len(ranks) > 1 else f'rank {ranks.pop()}'
+            raise ValueError(f'{part} LoRA of {m}: {shapes}: {why}, the config trains rank {rank}')
+
+
 def _check_where(where, allowed, part):
     if where not in allowed:
         raise NotImplementedError(f"{part} lora_cfg.where: {where!r} is not one of the reference's placements {allowed}")
@@ -90,6 +107,7 @@ class UNetLoRATrainer:
         probe_names = TrainEngine.lora_module_names.__get__(_NameProbe(self._topo, self.where))()
         if lora_state is None:
             lora_state = self._init_lora(probe_names)
+        check_lora_ranks(lora_state, self.rank, 'unet')
         self.engine = TrainEngine(self._sd, self.batch, H, W, lora=lora_state, lora_alpha=self.alpha,
                                   attn_reg_weight=self.attn_reg_weight, reg_full_identity=self.reg_full_identity,
                                   lr=self.unet_lr, device=self.device, where=self.where, **self._topo)
@@ -176,6 +194,7 @@ class UNetLoRATrainer:
         views = self.engine.lora_views
         if len(unet) != 2 * len(views):
             raise ValueError(f'checkpoint has {len(unet)} unet tensors, the model has {2 * len(views)} LoRA tensors')
+        check_lora_ranks(unet, self.rank, 'unet')
         self.engine.load_lora_state_dict(unet)
 
 
@@ -478,7 +497,11 @@ class EDLoRATrainer:
     def load_delta_state_dict(self, delta_state_dict):
         """trainer_edlora.py:315-356 (applied when the engines exist, i.e. at the first batch at the latest).  Unlike the
         reference, which skips the LoRA tensors of a group it does not train (no parameter name matches them), a checkpoint
-        carrying a LoRA for such a group is refused with ValueError rather than silently half-loaded."""
+        carrying a LoRA for such a group is refused with ValueError rather than silently half-loaded, and so is a LoRA
+        whose rank is not the configured rank of its group (check_lora_ranks), before any engine is touched."""
+        for part, on, rank in (('text_encoder', self.train_text, self.text_rank), ('unet', self.train_unet, self.unet_rank)):
+            if on:
+                check_lora_ranks(delta_state_dict.get(part) or {}, rank, part)
         if self.engine is None:
             self._loaded = delta_state_dict
         else:

@@ -53,7 +53,9 @@ def merge_lora_into_weight(original_state_dict, lora_state_dict, model_type, alp
             down = lora_state_dict[down_name].to(original_params.device)
             up = lora_state_dict[up_name].to(original_params.device)
             if len(original_params.shape) == 4:
-                lora_param = (up.squeeze() @ down.squeeze()).unsqueeze(-1).unsqueeze(-1)
+                # flatten, not the reference's squeeze: at rank 1 squeeze also drops the rank dimension, and up @ down
+                # becomes the dot product of two vectors added to every element of the weight
+                lora_param = (up.flatten(1) @ down.flatten(1)).unsqueeze(-1).unsqueeze(-1)
             else:
                 lora_param = up @ down
             new_state_dict[k] = original_params + alpha * lora_param

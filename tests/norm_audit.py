@@ -63,7 +63,8 @@ covered by using n + 8).
   dU = alpha dY^T t by (M + 16) u over the magnitudes plus the carried errors of s and t, then + d_* when accumulating.
 - attn_reg_group: cm is the mean of L heads x layers terms ((L H + 2) u); the statistics are checked against the launch's
   own cm: max and the tie / zero counts exactly, loss, S0, S1 over B N terms ((B N + 16) u).  attn_reg_grad: eight
-  roundings of each term and four of the product with k.  attn_reg_total: (ngroups + 2) u; NaN where the reference is.
+  roundings of each term and four of the product with k; with reg_full_identity also the rounding of x1 / M1 before
+  the target is subtracted (u |x1 / M1| twice: the difference cancels where the map is close to the target).  attn_reg_total: (ngroups + 2) u; NaN where the reference is.
 - flat_adamw_step: per element from the fp32 hyper-parameters passed: p (1 - lr wd) 3u, m 4u and v 5u of their terms,
   sqrt(v) min(e_v / (2 sqrt v), sqrt e_v) + u, the denominator, the step (lr / bc1) m / denom with 4u plus the carried
   errors; the row-norm mean of the embedding rows (read from the launch's updated params): (dim + 8) u / 2 + 2u per norm.
@@ -967,7 +968,11 @@ def _reference_training(rec):
         p0, q0 = g0 / M0, torch.where(x0 == M0, S0 / (M0 * M0 * T0), torch.zeros_like(x0))
         p1, q1 = g1 / M1, torch.where(x1 == M1, S1 / (M1 * M1 * T1), torch.zeros_like(x1))
         d = torch.stack([k * (p0 - q0), k * (p1 - q1)], -1)
-        eb = torch.stack([abs(k) * 8 * U32 * (p0.abs() + q0.abs()), abs(k) * 8 * U32 * (p1.abs() + q1.abs())], -1)
+        # full identity: x1 / M1 is rounded before the target is subtracted, and x1 / M1 - gt cancels where the map is
+        # close to the target, so that rounding is bounded by |x1 / M1|, not by |g1|
+        e_g1 = 2 * U32 * 2 * (x1 / M1).abs() / total if a['full'] else torch.zeros_like(x1)
+        eb = torch.stack([abs(k) * 8 * U32 * (p0.abs() + q0.abs()),
+                          abs(k) * (8 * U32 * (p1.abs() + q1.abs()) + e_g1 / M1)], -1)
         return {'gcols': (d, eb + 4 * U32 * d.abs())}
     if e == 'mos_attn_reg_total':
         ls = x['stats_all'][:, 5].double()
