@@ -684,7 +684,8 @@ def _check_lora_targets(params, path):
 
 
 def parse_new_concepts(concept_cfg):
-    """gradient_fusion.py:262-322: split every concept's `.pth` into embedding / text-encoder / cross-K/V / spatial parts."""
+    """gradient_fusion.py:262-322: split every concept's `.pth` into embedding / text-encoder / cross-K/V / spatial parts.
+    A concept embedding without 16 rows (a vanilla LoRA checkpoint) is refused here, naming the file."""
     import json
     if isinstance(concept_cfg, str):
         with open(concept_cfg, 'r') as f:
@@ -697,6 +698,11 @@ def parse_new_concepts(concept_cfg):
         model = torch.load(concept['lora_path'], map_location='cpu')['params']
         _check_lora_targets(model, concept['lora_path'])
         emb = model.get('new_concept_embedding')
+        for name, e in (emb or {}).items():
+            if e.shape[0] != NUM_CROSS_ATTENTION_LAYERS:
+                raise ValueError(f"{concept['lora_path']}: the embedding of {name} has {e.shape[0]} rows, gradient fusion "
+                                 f'takes ED-LoRA checkpoints ({NUM_CROSS_ATTENTION_LAYERS} layer-wise rows per concept); '
+                                 'a vanilla LoRA (enable_edlora: false) cannot be fused')
         embedding_list.append(emb if emb is not None and len(emb) != 0 else None)
         te = model.get('text_encoder')
         text_encoder_list.append(te if te is not None and len(te) != 0 else None)

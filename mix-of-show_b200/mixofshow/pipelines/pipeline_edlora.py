@@ -1,5 +1,8 @@
 """Drop-in for the reference's `mixofshow/pipelines/pipeline_edlora.py`: `bind_concept_prompt` and `EDLoRAPipeline`
-with the same constructor / `set_new_concept_cfg` / `set_controller` / `__call__` surface.
+with the same constructor / `set_new_concept_cfg` / `set_controller` / `__call__` surface, and the diffusers
+`StableDiffusionPipeline` the reference imports from the same module (test_edlora.py:16, train_edlora.py:18): the sampler
+of vanilla LoRA checkpoints (`convert_edlora(pipe, ckpt, enable_edlora=False, alpha)`), prompts encoded unbound, one CLIP
+pass per prompt, one [B, 77, 768] embedding for every cross-attention layer (the UNet's default processors).
 
 The denoise loop (reference :271-301) runs on the GPU engine: per step one captured UNet graph (CFG batch 2) and
 ONE fused kernel for CFG combine + DPM-Solver++(2M) update + re-duplication of the latents (`mos_cfg_dpmpp_step`).
@@ -41,16 +44,15 @@ def bind_concept_prompt(prompts, new_concept_cfg):
     return new_prompts
 
 
-class EDLoRAPipeline:
-    def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None, safety_checker=None,
-                 feature_extractor=None, requires_safety_checker: bool = False):
-        assert unet is not None, 'EDLoRAPipeline needs the GPU UNet'
-        revise_edlora_unet_attention_forward(unet)          # reference :93
+class _GPUPipeline:
+    """What both pipelines share: the components, `from_pretrained`'s loading and the denoise loop."""
+
+    def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None):
+        assert unet is not None, f'{type(self).__name__} needs the GPU UNet'
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.scheduler = scheduler if scheduler is not None else DPMSolverPP2M()
         # diffusers: 2 ** (len(vae.config.block_out_channels) - 1); 8 for SD1.5 (and when no VAE is attached)
         self.vae_scale_factor = 2 ** (len(vae.config.block_out_channels) - 1) if vae is not None else 8
-        self.new_concept_cfg = None
         self.device = torch.device('cuda')
 
     @classmethod
@@ -69,92 +71,43 @@ class EDLoRAPipeline:
             from transformers import CLIPTokenizer
             tokenizer = CLIPTokenizer.from_pretrained(pretrained_model_name_or_path, subfolder='tokenizer')
         pipe = cls(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler)
-        if os.path.exists(os.path.join(pretrained_model_name_or_path, 'new_concept_cfg.json')):   # a fused model
-            cfg = model_io.load_new_concept_cfg(pretrained_model_name_or_path)
-            model_io.ensure_concept_tokens(tokenizer, cfg)
-            pipe.set_new_concept_cfg(cfg)
+        pipe._loaded_from(pretrained_model_name_or_path)
         return pipe.to(device)
+
+    def _loaded_from(self, path):
+        """after `from_pretrained` has loaded the components (EDLoRAPipeline reads a fused model's concept config)"""
 
     def to(self, device):
         self.device = torch.device(device)
         return self
 
-    def set_new_concept_cfg(self, new_concept_cfg=None):
-        self.new_concept_cfg = new_concept_cfg
-
-    def set_controller(self, controller):
-        self.controller = controller
-        revise_edlora_unet_attention_controller_forward(self.unet, controller)
-
-    # reference :111-190
-    def _encode_prompt(self, prompt, new_concept_cfg, device, num_images_per_prompt, do_classifier_free_guidance,
-                       negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None):
-        assert num_images_per_prompt == 1, 'only support num_images_per_prompt=1 now'
+    @staticmethod
+    def _batch_size(prompt, prompt_embeds):
         if prompt is not None and isinstance(prompt, str):
-            batch_size = 1
-        elif prompt is not None and isinstance(prompt, list):
-            batch_size = len(prompt)
-        else:
-            batch_size = prompt_embeds.shape[0]
-        if prompt_embeds is None:
-            if self.tokenizer is None or self.text_encoder is None:
-                raise ValueError('no tokenizer / text_encoder supplied: pass prompt_embeds [B,16,77,768]')
-            prompt_extend = bind_concept_prompt(prompt, new_concept_cfg)
-            ids = self.tokenizer(prompt_extend, padding='max_length', max_length=self.tokenizer.model_max_length,
-                                 truncation=True, return_tensors='pt').input_ids
-            prompt_embeds = self.text_encoder(ids.to(device))[0]
-            prompt_embeds = prompt_embeds.reshape(batch_size, -1, *prompt_embeds.shape[1:])   # '(b n) m c -> b n m c'
-        prompt_embeds = prompt_embeds.to(device)
-        bs_embed, layer_num, seq_len, _ = prompt_embeds.shape
-        if do_classifier_free_guidance and negative_prompt_embeds is None:
-            if self.tokenizer is None or self.text_encoder is None:
-                raise ValueError('classifier-free guidance needs negative_prompt_embeds [B,77,768] when no text '
-                                 'encoder is supplied')
-            if negative_prompt is None:
-                uncond_tokens = [''] * batch_size
-            elif type(prompt) is not type(negative_prompt):
-                raise TypeError(f'`negative_prompt` should be the same type to `prompt`, but got '
-                                f'{type(negative_prompt)} != {type(prompt)}.')
-            elif isinstance(negative_prompt, str):
-                uncond_tokens = [negative_prompt]
-            elif batch_size != len(negative_prompt):
-                raise ValueError(f'`negative_prompt`: {negative_prompt} has batch size {len(negative_prompt)}, but '
-                                 f'`prompt`: {prompt} has batch size {batch_size}.')
-            else:
-                uncond_tokens = negative_prompt
-            ids = self.tokenizer(uncond_tokens, padding='max_length', max_length=seq_len, truncation=True,
-                                 return_tensors='pt').input_ids
-            negative_prompt_embeds = self.text_encoder(ids.to(device))[0]
-        if do_classifier_free_guidance:
-            seq_len = negative_prompt_embeds.shape[1]
-            negative_prompt_embeds = negative_prompt_embeds.to(device)
-            negative_prompt_embeds = negative_prompt_embeds.view(batch_size, 1, seq_len, -1).repeat(1, layer_num, 1, 1)
-            prompt_embeds = torch.cat([negative_prompt_embeds, prompt_embeds])
-        return prompt_embeds
+            return 1
+        if prompt is not None and isinstance(prompt, list):
+            return len(prompt)
+        return prompt_embeds.shape[0]
 
-    @torch.no_grad()
-    def __call__(self, prompt: Union[str, List[str]] = None, height: Optional[int] = None,
-                 width: Optional[int] = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
-                 negative_prompt=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
-                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
-                 negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = 'pil',
-                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None):
-        height = height or self.unet.config.sample_size * self.vae_scale_factor
-        width = width or self.unet.config.sample_size * self.vae_scale_factor
-        if height % 8 != 0 or width % 8 != 0:
-            raise ValueError(f'`height` and `width` have to be divisible by 8 but are {height} and {width}.')
-        if prompt is not None and isinstance(prompt, str):
-            batch_size = 1
-        elif prompt is not None and isinstance(prompt, list):
-            batch_size = len(prompt)
-        else:
-            batch_size = prompt_embeds.shape[0]
+    def _uncond_tokens(self, prompt, negative_prompt, batch_size):
+        """reference :161-181 (diffusers' checks on negative_prompt)"""
+        if negative_prompt is None:
+            return [''] * batch_size
+        if type(prompt) is not type(negative_prompt):
+            raise TypeError(f'`negative_prompt` should be the same type to `prompt`, but got '
+                            f'{type(negative_prompt)} != {type(prompt)}.')
+        if isinstance(negative_prompt, str):
+            return [negative_prompt]
+        if batch_size != len(negative_prompt):
+            raise ValueError(f'`negative_prompt`: {negative_prompt} has batch size {len(negative_prompt)}, but '
+                             f'`prompt`: {prompt} has batch size {batch_size}.')
+        return negative_prompt
+
+    def _denoise(self, prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator, latents,
+                 output_type, return_dict, callback, callback_steps, cross_attention_kwargs):
+        """reference :262-322 from the timesteps to the decoded images; `prompt_embeds` carries the CFG halves"""
         device = self.device
         do_cfg = guidance_scale > 1.0
-        assert self.new_concept_cfg is not None
-        prompt_embeds = self._encode_prompt(prompt, self.new_concept_cfg, device, num_images_per_prompt, do_cfg,
-                                            negative_prompt, prompt_embeds=prompt_embeds,
-                                            negative_prompt_embeds=negative_prompt_embeds)
         self.scheduler.set_timesteps(num_inference_steps, device=device)
         timesteps = [int(t) for t in self.scheduler.timesteps]
         h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
@@ -200,3 +153,137 @@ class EDLoRAPipeline:
         if not return_dict:
             return (image)
         return SimpleNamespace(images=image, nsfw_content_detected=None)
+
+
+class EDLoRAPipeline(_GPUPipeline):
+    def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None, safety_checker=None,
+                 feature_extractor=None, requires_safety_checker: bool = False):
+        assert unet is not None, 'EDLoRAPipeline needs the GPU UNet'
+        revise_edlora_unet_attention_forward(unet)          # reference :93
+        super().__init__(vae, text_encoder, tokenizer, unet, scheduler)
+        self.new_concept_cfg = None
+
+    def _loaded_from(self, pretrained_model_name_or_path):
+        import os
+        from mixofshow.utils import model_io
+        if os.path.exists(os.path.join(pretrained_model_name_or_path, 'new_concept_cfg.json')):   # a fused model
+            cfg = model_io.load_new_concept_cfg(pretrained_model_name_or_path)
+            model_io.ensure_concept_tokens(self.tokenizer, cfg)
+            self.set_new_concept_cfg(cfg)
+
+    def set_new_concept_cfg(self, new_concept_cfg=None):
+        self.new_concept_cfg = new_concept_cfg
+
+    def set_controller(self, controller):
+        self.controller = controller
+        revise_edlora_unet_attention_controller_forward(self.unet, controller)
+
+    # reference :111-190
+    def _encode_prompt(self, prompt, new_concept_cfg, device, num_images_per_prompt, do_classifier_free_guidance,
+                       negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None):
+        assert num_images_per_prompt == 1, 'only support num_images_per_prompt=1 now'
+        batch_size = self._batch_size(prompt, prompt_embeds)
+        if prompt_embeds is None:
+            if self.tokenizer is None or self.text_encoder is None:
+                raise ValueError('no tokenizer / text_encoder supplied: pass prompt_embeds [B,16,77,768]')
+            prompt_extend = bind_concept_prompt(prompt, new_concept_cfg)
+            ids = self.tokenizer(prompt_extend, padding='max_length', max_length=self.tokenizer.model_max_length,
+                                 truncation=True, return_tensors='pt').input_ids
+            prompt_embeds = self.text_encoder(ids.to(device))[0]
+            prompt_embeds = prompt_embeds.reshape(batch_size, -1, *prompt_embeds.shape[1:])   # '(b n) m c -> b n m c'
+        prompt_embeds = prompt_embeds.to(device)
+        bs_embed, layer_num, seq_len, _ = prompt_embeds.shape
+        if do_classifier_free_guidance and negative_prompt_embeds is None:
+            if self.tokenizer is None or self.text_encoder is None:
+                raise ValueError('classifier-free guidance needs negative_prompt_embeds [B,77,768] when no text '
+                                 'encoder is supplied')
+            uncond_tokens = self._uncond_tokens(prompt, negative_prompt, batch_size)
+            ids = self.tokenizer(uncond_tokens, padding='max_length', max_length=seq_len, truncation=True,
+                                 return_tensors='pt').input_ids
+            negative_prompt_embeds = self.text_encoder(ids.to(device))[0]
+        if do_classifier_free_guidance:
+            seq_len = negative_prompt_embeds.shape[1]
+            negative_prompt_embeds = negative_prompt_embeds.to(device)
+            negative_prompt_embeds = negative_prompt_embeds.view(batch_size, 1, seq_len, -1).repeat(1, layer_num, 1, 1)
+            prompt_embeds = torch.cat([negative_prompt_embeds, prompt_embeds])
+        return prompt_embeds
+
+    @torch.no_grad()
+    def __call__(self, prompt: Union[str, List[str]] = None, height: Optional[int] = None,
+                 width: Optional[int] = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
+                 negative_prompt=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = 'pil',
+                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None):
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        if height % 8 != 0 or width % 8 != 0:
+            raise ValueError(f'`height` and `width` have to be divisible by 8 but are {height} and {width}.')
+        batch_size = self._batch_size(prompt, prompt_embeds)
+        device = self.device
+        do_cfg = guidance_scale > 1.0
+        assert self.new_concept_cfg is not None
+        prompt_embeds = self._encode_prompt(prompt, self.new_concept_cfg, device, num_images_per_prompt, do_cfg,
+                                            negative_prompt, prompt_embeds=prompt_embeds,
+                                            negative_prompt_embeds=negative_prompt_embeds)
+        return self._denoise(prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator,
+                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs)
+
+
+class StableDiffusionPipeline(_GPUPipeline):
+    """diffusers' StableDiffusionPipeline on the GPU engines, the sampler of vanilla LoRA: `from_pretrained` and `__call__`
+    with EDLoRAPipeline's arguments; prompts are tokenized as written (no binding), CLIP runs once per prompt, and
+    `prompt_embeds` / `negative_prompt_embeds` are [B, 77, 768].  The UNet keeps its default attention processors and
+    reads that one embedding in all 16 cross-attention layers.  As in diffusers there is no `set_new_concept_cfg`: the
+    concept tokens `<new{k}>` that `convert_edlora(pipe, ckpt, enable_edlora=False, alpha)` adds go into the prompt
+    literally."""
+
+    def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet=None, scheduler=None, safety_checker=None,
+                 feature_extractor=None, requires_safety_checker: bool = False):
+        super().__init__(vae, text_encoder, tokenizer, unet, scheduler)
+
+    def _encode_prompt(self, prompt, device, num_images_per_prompt, do_classifier_free_guidance, negative_prompt=None,
+                       prompt_embeds=None, negative_prompt_embeds=None):
+        """diffusers StableDiffusionPipeline._encode_prompt: [uncond; cond] [2B, 77, 768] with CFG, [B, 77, 768] without"""
+        assert num_images_per_prompt == 1, 'only support num_images_per_prompt=1 now'
+        batch_size = self._batch_size(prompt, prompt_embeds)
+        if prompt_embeds is None:
+            if self.tokenizer is None or self.text_encoder is None:
+                raise ValueError('no tokenizer / text_encoder supplied: pass prompt_embeds [B,77,768]')
+            prompts = [prompt] if isinstance(prompt, str) else list(prompt)
+            ids = self.tokenizer(prompts, padding='max_length', max_length=self.tokenizer.model_max_length,
+                                 truncation=True, return_tensors='pt').input_ids
+            prompt_embeds = self.text_encoder(ids.to(device))[0]
+        prompt_embeds = prompt_embeds.to(device)
+        if prompt_embeds.ndim != 3:
+            raise ValueError(f'prompt_embeds must be [B, 77, 768], got {tuple(prompt_embeds.shape)}')
+        if not do_classifier_free_guidance:
+            return prompt_embeds
+        if negative_prompt_embeds is None:
+            if self.tokenizer is None or self.text_encoder is None:
+                raise ValueError('classifier-free guidance needs negative_prompt_embeds [B,77,768] when no text '
+                                 'encoder is supplied')
+            uncond_tokens = self._uncond_tokens(prompt, negative_prompt, batch_size)
+            ids = self.tokenizer(uncond_tokens, padding='max_length', max_length=prompt_embeds.shape[1], truncation=True,
+                                 return_tensors='pt').input_ids
+            negative_prompt_embeds = self.text_encoder(ids.to(device))[0]
+        negative_prompt_embeds = negative_prompt_embeds.to(device).reshape(prompt_embeds.shape)
+        return torch.cat([negative_prompt_embeds, prompt_embeds])
+
+    @torch.no_grad()
+    def __call__(self, prompt: Union[str, List[str]] = None, height: Optional[int] = None,
+                 width: Optional[int] = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
+                 negative_prompt=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
+                 latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = 'pil',
+                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None):
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        if height % 8 != 0 or width % 8 != 0:
+            raise ValueError(f'`height` and `width` have to be divisible by 8 but are {height} and {width}.')
+        batch_size = self._batch_size(prompt, prompt_embeds)
+        prompt_embeds = self._encode_prompt(prompt, self.device, num_images_per_prompt, guidance_scale > 1.0,
+                                            negative_prompt, prompt_embeds=prompt_embeds,
+                                            negative_prompt_embeds=negative_prompt_embeds)
+        return self._denoise(prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator,
+                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs)

@@ -16,7 +16,13 @@ the GPU VAE engine, :203-204) or already encoded latents.
 upstream).
 
 LoRA placement (`lora_cfg.where`, trainer_edlora.py:100-133): the UNet takes `Attention` or `Transformer2DModel`, the text
-encoder `CLIPAttention` or `CLIPEncoderLayer`, in any combination."""
+encoder `CLIPAttention` or `CLIPEncoderLayer`, in any combination.
+
+Vanilla LoRA (`enable_edlora: false`, trainer_edlora.py:156-160, :220-234): one token `<new{k}>` and one embedding row per
+concept word, prompts tokenized as written (no `bind_concept_prompt`), one text-encoder pass per sample, and the one
+[b, 77, 768] embedding shared by all 16 cross-attention layers (TrainEngine(shared_ehs=True)).  A concept row only receives
+a gradient when a prompt contains its `<new{k}>` token literally: a `replace_mapping` such as `<TOK>: <potter1> <potter2>`
+does not produce those tokens, so with it the rows stay where they were initialised, as in the reference."""
 import math
 import re
 
@@ -26,8 +32,10 @@ from mos_b200.clip_train_engine import CLIP_WHERE
 from mos_b200.engine import ehs_to_layer_major
 from mos_b200.train_engine import UNET_WHERE, TrainEngine
 
-VANILLA_LORA_UNSUPPORTED = ('enable_edlora=False (vanilla LoRA with one embedding per concept) is not built on the GPU '
-                            'path: the cross-attention kernels take layer-wise embeddings')
+VANILLA_LORA_UNSUPPORTED = ('enable_edlora=False (vanilla LoRA) checkpoints cannot be sampled by EDLoRAPipeline, so neither '
+                            'test_edlora.py nor val.val_during_save takes them (the reference fails there too): sample '
+                            'a lora_model-*.pth with StableDiffusionPipeline.from_pretrained(...) and '
+                            'convert_edlora(pipe, ckpt, enable_edlora=False, alpha=...)')
 
 
 FINETUNE_GROUPS = ('text_embedding', 'text_encoder', 'unet')
@@ -220,10 +228,8 @@ class EDLoRATrainer:
                  enable_xformers=False, gradient_checkpoint=False, *, tokenizer=None, latent_size=(64, 64), device='cuda',
                  seed=0):
         from mixofshow.utils import model_io
-        if not enable_edlora:
-            raise NotImplementedError(VANILLA_LORA_UNSUPPORTED)
         self.device = torch.device(device)
-        self.enable_edlora = True
+        self.enable_edlora = bool(enable_edlora)
         self.unet = model_io.load_unet(pretrained_path)                               # :44
         self.text_encoder = model_io.load_text_encoder(pretrained_path, device=device)   # :41
         if tokenizer is None:
@@ -234,7 +240,8 @@ class EDLoRATrainer:
         self.vae = model_io.load_vae(pretrained_path, device=device) if os.path.isdir(os.path.join(pretrained_path, 'vae')) \
             else None                                                                     # :39
         self._gen = torch.Generator(device='cpu').manual_seed(seed)
-        self.new_concept_cfg = self.init_new_concept(new_concept_token, initializer_token, enable_edlora=True)   # :55
+        self.new_concept_cfg = self.init_new_concept(new_concept_token, initializer_token,
+                                                     enable_edlora=self.enable_edlora)   # :55
         self.attn_reg_weight = attn_reg_weight
         self.reg_full_identity = reg_full_identity
         self.noise_offset = noise_offset
@@ -248,7 +255,7 @@ class EDLoRATrainer:
 
     # ------------------------------------------------------------------------------------------ new concept tokens
     def init_new_concept(self, new_concept_tokens, initializer_tokens, enable_edlora=True):
-        """trainer_edlora.py:144-194: 16 tokens `<new{k}>` per concept word, embedding rows initialised from
+        """trainer_edlora.py:144-194: 16 tokens `<new{k}>` per concept word (1 without ED-LoRA), embedding rows initialised from
         `<rand-sigma>` or from an existing single token."""
         new_concept_cfg = {}
         new_concept_tokens = new_concept_tokens.split('+')
@@ -385,8 +392,9 @@ class EDLoRATrainer:
         self.engine = TrainEngine(usd, batch, H, W, lora=ulora if self.train_unet else None, lora_alpha=self.unet_alpha,
                                   attn_reg_weight=self.attn_reg_weight, reg_full_identity=self.reg_full_identity,
                                   state=self.state, state_offset=self.state.group_end[1], text_grad=text_grad,
-                                  device=self.device, where=self.unet_where or UNET_WHERE[0], **topo)
-        n_x = len(self.engine.xattn_names)
+                                  device=self.device, where=self.unet_where or UNET_WHERE[0],
+                                  shared_ehs=not self.enable_edlora, **topo)
+        n_x = len(self.engine.xattn_names) if self.enable_edlora else 1      # text sequences per sample
         if text_grad:
             self.text_engine = CLIPTrainEngine(tsd, n_x * batch, lora=tlora if self.train_text else None,
                                                lora_alpha=self.text_alpha, concept_token_ids=ids, state=self.state,
@@ -422,6 +430,23 @@ class EDLoRATrainer:
         n_x = ids.shape[0] // b
         return ids, ids.view(b, n_x, -1).permute(1, 0, 2).reshape(n_x * b, -1).contiguous()
 
+    def tokenize(self, prompts):
+        """vanilla LoRA (:220-231 without the binding): prompts (b strings) -> token ids [b, 77], as written"""
+        return self.tokenizer(list(prompts), padding='max_length', max_length=self.tokenizer.model_max_length,
+                              truncation=True, return_tensors='pt').input_ids
+
+    def concept_token_positions(self, ids, b):
+        """trainer_edlora.py:270-279: the positions of the concept tokens in each sample's first id row (ids [(b l), 77],
+        l = 16 layer prompts with ED-LoRA, 1 without); the regulariser needs exactly two per sample"""
+        concept = set(int(i) for i in self.get_all_concept_token_ids())
+        pos = []
+        for text in ids.view(b, -1, ids.shape[-1]):
+            p = [i for i in range(text.shape[-1]) if int(text[0][i]) in concept]
+            if len(p) != 2:
+                raise ValueError(f'cal_attn_reg assumes exactly two concept tokens per prompt (:298), found {len(p)}')
+            pos.append(p)
+        return pos
+
     def forward(self, images, prompts, masks, img_masks, noise=None, timesteps=None, accumulate=False):
         """trainer_edlora.py:202-261.  `images`: [b,3,H,W] in [-1,1] (encoded by the GPU VAE, :203-204) or already encoded
         latents [b,4,h,w] (x 0.18215).  Runs forward + loss + backward of the whole step (text encoder and UNet) and returns
@@ -444,19 +469,14 @@ class EDLoRATrainer:
                 noise = noise + self.noise_offset * torch.randn((b, latents.shape[1], 1, 1), generator=self._gen)
         if timesteps is None:
             timesteps = torch.randint(0, 1000, (b,), generator=self._gen)
-        ids, ids_lm = self.tokenize_layerwise(prompts)
+        if self.enable_edlora:
+            ids, ids_lm = self.tokenize_layerwise(prompts)
+        else:
+            ids = ids_lm = self.tokenize(prompts)
         n_x = len(self.engine.xattn_names)
-        if ids.shape[0] // b != n_x:          # a smaller topology uses the first n_x layer prompts of every sample
+        if self.enable_edlora and ids.shape[0] // b != n_x:          # a smaller topology uses the first n_x layer prompts of every sample
             ids_lm = ids.view(b, -1, ids.shape[-1])[:, :n_x].permute(1, 0, 2).reshape(n_x * b, -1).contiguous()
-        pos = None
-        if self.attn_reg_weight is not None:
-            concept = set(int(i) for i in self.get_all_concept_token_ids())
-            pos = []
-            for text in ids.view(b, -1, ids.shape[-1]):
-                p = [i for i in range(text.shape[-1]) if int(text[0][i]) in concept]        # :270-279
-                if len(p) != 2:
-                    raise ValueError(f'cal_attn_reg assumes exactly two concept tokens per prompt (:298), found {len(p)}')
-                pos.append(p)
+        pos = self.concept_token_positions(ids, b) if self.attn_reg_weight is not None else None
         loss_mask = masks if self.use_mask_loss else img_masks
         dev = self.device
         out = self.engine.forward_backward(latents.to(dev), noise.to(dev), timesteps.to(dev), None, masks.to(dev),

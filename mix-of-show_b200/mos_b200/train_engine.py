@@ -17,6 +17,12 @@ runs the full dX chain down to d(text embeddings) with no LoRA-gradient or LoRA-
 backward packs.  The text encoder is attached with `attach_text_engine`: a training CLIPTrainEngine (text_grad=True) or a
 frozen CLIPTextEngine whose forward runs inside the same captured step (text_grad=False: no d(text embeddings) and no text
 K / V dX GEMMs).
+
+With `shared_ehs=True` (vanilla LoRA, the reference's `enable_edlora: false`, trainer_edlora.py:220-234) every
+cross-attention layer reads ONE text embedding: `in_ehs` is [1, B, 77, 768] instead of the layer-major [16, B, 77, 768],
+the text encoder runs over B sequences, and d(text embedding) is the sum over the 16 layers of dK_l (W_k + a U_k D_k) +
+dV_l (W_v + a U_v D_v), accumulated in fp32 by the GEMM's fp32 output path (`accumulate`) in the backward's fixed layer
+order (so the step stays bit-reproducible) and rounded to bf16 once for the text encoder's backward.
 """
 import math
 
@@ -39,16 +45,20 @@ def _key(t):
 
 class TrainEngine(UNetEngine):
     def __init__(self, state_dict, batch, height, width, *, lora, lora_alpha=1.0, attn_reg_weight=0.01,
-                 reg_full_identity=True, lr=1e-4, state=None, state_offset=0, text_grad=False, where='Attention', **kw):
+                 reg_full_identity=True, lr=1e-4, state=None, state_offset=0, text_grad=False, where='Attention',
+                 shared_ehs=False, **kw):
         """where: the LoRA placement (UNET_WHERE); `lora` must hold a pair for every module of lora_module_names(), or be
         None for a frozen UNet (only with a shared `state`: the text encoder trains).
         state / state_offset: a shared dp.FlatTrainState (and the offset of the UNet-LoRA block in it) when the text
         encoder is trained in the same step (clip_train_engine.CLIPTrainEngine); None = a private state.
         text_grad: also produce d loss / d(text embeddings) into `self.d_ehs` (bf16 [16 * B * 77, 800], layer-major rows =
-        the layout of `in_ehs`; the first 768 columns are the gradient) for the text encoder's backward."""
+        the layout of `in_ehs`; the first 768 columns are the gradient) for the text encoder's backward.
+        shared_ehs: one text embedding for all cross-attention layers (vanilla LoRA): `in_ehs` [1, B, 77, 768], `d_ehs`
+        bf16 [B * 77, 800] rounded from the fp32 layer sum `d_ehs_f32` [B * 77, 800]."""
         if where not in UNET_WHERE:
             raise ValueError(f'where: {where!r} is not one of {UNET_WHERE}')
         self.where = where
+        self.shared_ehs = bool(shared_ehs)
         self.use_train_graph = bool(kw.pop('use_graph', True))
         self._ext_state, self._state_off, self.text_grad = state, int(state_offset), bool(text_grad)
         self.tgraph = None
@@ -79,6 +89,15 @@ class TrainEngine(UNetEngine):
         """SD1.5 scaled-linear schedule (scheduler config of the checkpoint the reference loads, trainer_edlora.py:43)."""
         betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, n, dtype=torch.float32) ** 2
         return torch.cumprod(1.0 - betas, dim=0)
+
+    def _alloc_io(self):
+        super()._alloc_io()
+        if self.shared_ehs:
+            self.in_ehs = torch.zeros(1, self.B, self.n_text, self.cross_dim, device=self.dev, dtype=self.ACT)
+
+    def _ehs(self, xidx):
+        """the text embedding cross-attention layer xidx reads: its own slice, or the shared one"""
+        return self.in_ehs[0 if self.shared_ehs else xidx]
 
     # ------------------------------------------------------------------------------------------ LoRA state
     def lora_module_names(self):
@@ -274,10 +293,12 @@ class TrainEngine(UNetEngine):
                 Wp[:Wt.shape[0]] = Wt
                 Wt = Wp
             self.wb[bk]['W'] = Wt.contiguous()
-        self.d_ehs = None
+        self.d_ehs = self.d_ehs_f32 = None
         if self.text_grad:
-            self.d_ehs = torch.zeros(len(self.xattn_names) * self.B * self.n_text, _r(self.cross_dim, 160), device=self.dev,
-                                     dtype=BF16)
+            rows = (1 if self.shared_ehs else len(self.xattn_names)) * self.B * self.n_text
+            self.d_ehs = torch.zeros(rows, _r(self.cross_dim, 160), device=self.dev, dtype=BF16)
+            if self.shared_ehs:
+                self.d_ehs_f32 = torch.zeros(rows, _r(self.cross_dim, 160), device=self.dev, dtype=F32)
 
     # ------------------------------------------------------------------------------------------ buffers
     def tb(self, tag, shape, dtype=BF16, zero=False):
@@ -422,6 +443,14 @@ class TrainEngine(UNetEngine):
         ops.lora_grad(x, dy, D, U, self.lora_alpha, self._lg_ws(M, K, N), gD, gU, M=M, K=K, N=N, ldx=ldx, lddy=lddy,
                       accumulate=self._accumulate)
 
+    def _gemm_f32(self, A, ent, out, *, M, lda, accumulate):
+        """out (fp32) = [out +] A @ ent^T (+ its LoRA term): one launch, no split-K (the fp32 output path takes none)"""
+        kw = {}
+        if 'lora_down' in ent:
+            kw = dict(lora_down=ent['lora_down'], lora_up=ent['lora_up'], lora_seg=ent['lora_seg'])
+        ops.gemm(A, ent['W'], out, M=M, lda=lda, out_f32=True, accumulate=accumulate, **kw)
+        self.launches += 1
+
     def _attn_bwd(self, Q, K, V, ao, lse, dO, dq, dk, dv, N, nk, d, pcols=None, gcols=None):
         B, Hh = self.B, self.heads
         BH = B * Hh
@@ -477,11 +506,16 @@ class TrainEngine(UNetEngine):
         gcols = self.gcols_by_layer.get(xidx)
         self._attn_bwd(S['Q2'], Kc, Vc, S['ao2'], S['lse2'], dO, dq, dkv[:, :C], dkv[:, C:], N, T, d,
                        pcols=S['pcols'] if gcols is not None else None, gcols=gcols)
-        ehs = self.in_ehs[xidx].reshape(B * T, self.cross_dim)
+        ehs = self._ehs(xidx).reshape(B * T, self.cross_dim)
         self._lora_grad(a2 + 'to_q', S['ln2'], dq, M)
         self._lora_grad(a2 + 'to_k', ehs, dkv[:, :C], B * T, lddy=2 * C)
         self._lora_grad(a2 + 'to_v', ehs, dkv[:, C:], B * T, lddy=2 * C)
-        if self.d_ehs is not None:      # d(text embedding of layer xidx) = dK (W_k + a U_k D_k) + dV (W_v + a U_v D_v)
+        if self.d_ehs_f32 is not None:  # shared embedding: the same two products, added to the fp32 layer sum
+            self._gemm_f32(dkv[:, :C], self.wb[a2 + 'to_k'], self.d_ehs_f32, M=B * T, lda=2 * C,
+                           accumulate=not self._dehs_first)
+            self._gemm_f32(dkv[:, C:], self.wb[a2 + 'to_v'], self.d_ehs_f32, M=B * T, lda=2 * C, accumulate=True)
+            self._dehs_first = False
+        elif self.d_ehs is not None:    # d(text embedding of layer xidx) = dK (W_k + a U_k D_k) + dV (W_v + a U_v D_v)
             dst = self.d_ehs[xidx * B * T:(xidx + 1) * B * T]
             self.gemm(dkv[:, :C], self.wb[a2 + 'to_k'], dst, M=B * T, lda=2 * C)
             self.gemm(dkv[:, C:], self.wb[a2 + 'to_v'], dst, M=B * T, lda=2 * C, residual=dst)
@@ -522,7 +556,7 @@ class TrainEngine(UNetEngine):
         self.kvt = {}
         chans = self._xattn_channels()
         for xidx, (an, C) in enumerate(zip(self.xattn_names, chans)):
-            self.kvt[xidx] = self._cross_kv_train(an[:-len('.attn2')], self.in_ehs[xidx], C, xidx)
+            self.kvt[xidx] = self._cross_kv_train(an[:-len('.attn2')], self._ehs(xidx), C, xidx)
         si = 0
         x = self._skip_slot(si)
         ops.conv_in(self.in_latents, self.w['conv_in'][0], self.w['conv_in'][1], x, ldy=x.stride(0))
@@ -658,6 +692,7 @@ class TrainEngine(UNetEngine):
         d_fin = self.tb('g.final', (M, c0))
         ops.groupnorm_bwd(fin, d_fn, g, b, d_fin, self._gnws(), B=B, HW=h * w, C=c0, eps=1e-5, silu=True)
         grads = {_key(fin): d_fin}
+        self._dehs_first = True
         for e in reversed(self.trace):
             kind = e[0]
             if kind == 'resnet':
@@ -684,14 +719,17 @@ class TrainEngine(UNetEngine):
                 ops.upsample2x_bwd(d_up, dX, B=B, H=h, W=w, C=c)
                 self._deposit(grads, x, dX)
         self._leftover = grads      # only the conv_in output gradient remains (the latents need no gradient)
+        if self.d_ehs_f32 is not None:  # the fp32 layer sum -> bf16, once (a one-slice "split-K" reduction)
+            ops.splitk_finalize(self.d_ehs_f32, 1, self.d_ehs.shape[0], self.d_ehs.shape[1], self.d_ehs)
+            self.launches += 1
 
     # ------------------------------------------------------------------------------------------ public API
     def attach_text_engine(self, text_engine):
-        """Run the text encoder in the same (captured) step: `text_engine` (over 16 * B layer-major sequences) writes its
-        last hidden state straight into `in_ehs` before the UNet forward.  With text_grad=True it is a
+        """Run the text encoder in the same (captured) step: `text_engine` (over 16 * B layer-major sequences, B with
+        shared_ehs) writes its last hidden state straight into `in_ehs` before the UNet forward.  With text_grad=True it is a
         clip_train_engine.CLIPTrainEngine that consumes `d_ehs` after the UNet backward; with text_grad=False a frozen
         clip_engine.CLIPTextEngine that runs its forward only."""
-        assert text_engine.n_seq == len(self.xattn_names) * self.B
+        assert text_engine.n_seq == (1 if self.shared_ehs else len(self.xattn_names)) * self.B
         assert not self.text_grad or hasattr(text_engine, 'backward'), "text_grad needs a training text engine"
         self.text = text_engine
         self._tgraphs = {}
@@ -699,12 +737,12 @@ class TrainEngine(UNetEngine):
     def forward_backward(self, latents, noise, timesteps, ehs_layers, masks, loss_mask=None, token_pos=None,
                          accumulate=False, text_ids=None):
         """One forward + loss + backward.  latents (x0) / noise fp32 [B,4,H,W]; timesteps int [B]; ehs_layers bf16
-        [16,B,77,768]; masks / loss_mask [B,1,H,W] (trainer_edlora.py:246-252); token_pos: B pairs of concept-token
+        [16,B,77,768] (shared_ehs: [B,77,768]); masks / loss_mask [B,1,H,W] (trainer_edlora.py:246-252); token_pos: B pairs of concept-token
         positions (:270-279).  Returns the device tensor [total loss, attention loss]."""
         self.t_i32.copy_(timesteps.to(self.dev, torch.int32))
         self.in_t.copy_(timesteps.to(self.dev, F32))
         if getattr(self, 'text', None) is not None:
-            self.text.set_ids(text_ids)                              # layer-major [16 * B, 77] token ids
+            self.text.set_ids(text_ids)              # layer-major [16 * B, 77] token ids ([B, 77] with shared_ehs)
         else:
             self.in_ehs.copy_(ehs_layers)
         self.target.copy_(noise)                                     # prediction_type 'epsilon' (:241-242)

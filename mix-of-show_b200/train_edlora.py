@@ -17,6 +17,11 @@ Data: the image pipeline (LoraDataset transforms, VAE encoder) is outside the ho
 Checkpoints and validation (train_edlora.py:157-189): `edlora_model-{step}.pth` every `logger.save_checkpoint_freq` steps
 and `edlora_model-latest.pth` at the end; with `val.val_during_save`, each saved checkpoint is sampled over
 `datasets.val_vis` for every alpha of `val.alpha_list` by test_edlora.py's `visual_validation`, sharded across ranks.
+
+With `models.enable_edlora: false` the trainer is vanilla LoRA (one embedding per concept) and the checkpoints are
+`lora_model-{step}.pth` / `lora_model-latest.pth` (train_edlora.py:166-168).  Such a checkpoint cannot be validated through
+EDLoRAPipeline, so `val.val_during_save: true` is refused at startup, before anything is built or trained (the reference
+only fails after its first checkpoint).
 """
 import functools
 import os
@@ -136,6 +141,7 @@ def main(argv=None):
     args = parser.parse_args(argv)
     with open(args.opt) as f:
         opt = yaml.safe_load(f)
+    check_options(opt)
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
@@ -178,12 +184,25 @@ def main(argv=None):
     return losses
 
 
+def check_options(opt):
+    """Refuses (NotImplementedError) what the run could only fail at later: validating vanilla LoRA checkpoints."""
+    from mixofshow.pipelines.trainer_edlora import VANILLA_LORA_UNSUPPORTED
+    if not opt['models'].get('enable_edlora', True) and (opt.get('val') or {}).get('val_during_save'):
+        raise NotImplementedError(f'val.val_during_save: {VANILLA_LORA_UNSUPPORTED}; set val_during_save: false')
+
+
+def checkpoint_path(opt, global_step):
+    """train_edlora.py:166-168: `edlora_model-{step}.pth`, or `lora_model-{step}.pth` for vanilla LoRA"""
+    lora_type = 'edlora' if opt['models'].get('enable_edlora', True) else 'lora'
+    return os.path.join(opt['path']['models'], f'{lora_type}_model-{global_step}.pth')
+
+
 def save_and_validation(trainer, opt, val_dataset, global_step, *, rank=0, world=1, log=print):
-    """train_edlora.py:165-189: rank 0 writes `edlora_model-{global_step}.pth`; then every rank waits for it and, when
+    """train_edlora.py:165-189: rank 0 writes `checkpoint_path(opt, global_step)`; then every rank waits for it and, when
     `val_dataset` is given, samples its share of the set from that file for each alpha of `val.alpha_list` into
     `Iters-{global_step}_Alpha-{alpha}` (test_edlora.py's `visual_validation`).  The pipeline is loaded fresh from the
     pretrained directory and the checkpoint file, so validation reads nothing of the trainer."""
-    save_path = os.path.join(opt['path']['models'], f'edlora_model-{global_step}.pth')
+    save_path = checkpoint_path(opt, global_step)
     if rank == 0:
         os.makedirs(opt['path']['models'], exist_ok=True)
         torch.save({'params': trainer.delta_state_dict()}, save_path)
