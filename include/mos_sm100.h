@@ -148,10 +148,15 @@ int mos_conv_in(const float* x, int32_t B, int32_t Cin, int32_t H, int32_t W, co
 int mos_conv_out(const void* x, int32_t B, int32_t H, int32_t W, int32_t C, const float* w, const float* bias,
                  int32_t Cout, float* y, int32_t act_dtype, void* stream);
 
-/* Upsample2D nearest x2: NHWC bf16 [B, H, W, ldx] -> contiguous [B, 2H, 2W, C]. */
-int mos_upsample2x(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, void* y, void* stream);
-/* Downsample2D (3x3, stride 2) im2col: NHWC 16-bit -> [B*H/2*W/2, 9*C] for mos_gemm_bf16.  pad = 1: symmetric padding 1
- * (UNet Downsample2D); pad = 0: the VAE encoder's variant (F.pad (0,1,0,1) then no padding: taps start at 2*ho). */
+/* Upsample2D nearest: NHWC 16-bit [B, H, W, ldx] -> contiguous [B, Ho, Wo, C].  Ho = 2H, Wo = 2W is the x2 upsample
+ * (source pixel dst >> 1); any other size is diffusers' output_size path (the size of the skip an up block meets when a
+ * latent side is not a multiple of 2^(levels - 1)), with PyTorch upsample_nearest2d's source index
+ * min(floor(dst * (float)in / out), in - 1) in fp32. */
+int mos_upsample2x(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, void* y, int32_t Ho, int32_t Wo,
+                   void* stream);
+/* Downsample2D (3x3, stride 2) im2col: NHWC 16-bit -> [B*Ho*Wo, 9*C] for mos_gemm_bf16.  pad = 1: symmetric padding 1
+ * (UNet Downsample2D, any H, W: Ho = ceil(H/2), Wo = ceil(W/2)); pad = 0: the VAE encoder's variant (F.pad (0,1,0,1) then
+ * no padding: taps start at 2*ho; even H, W only, Ho = H/2, Wo = W/2). */
 int mos_im2col_s2(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, int32_t pad, void* col,
                   void* stream);
 /* x[m, :C] += r[m, :C] (T2I-Adapter residuals, pipeline_regionally_t2iadapter.py:565). */

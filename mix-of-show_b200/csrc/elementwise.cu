@@ -183,12 +183,39 @@ __global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ x, long long
   *reinterpret_cast<uint4*>(y + pix * C + o * 8) = u;
 }
 
-// col[(b,ho,wo), tap*C + c] = x[b, 2ho+kh-1, 2wo+kw-1, c] (zero outside): Downsample2D conv 3x3 / stride 2 / pad 1
+// y[b, ho, wo, :] = x[b, sh(ho), sw(wo), :]: F.interpolate(size=(Ho, Wo), mode='nearest') with PyTorch's source index
+// rule, src = min(floor(dst * (in / out)), in - 1) in fp32 (dst >> 1 when out = 2 in).  diffusers' Upsample2D takes this
+// path (output_size) when a latent side is not a multiple of 2^(levels - 1): each level is ceil(in / 2) of the one above.
+__device__ __forceinline__ int nearest_src(int dst, int in, int out) {
+  if (out == 2 * in) return dst >> 1;
+  return min((int)floorf(__fmul_rn((float)dst, __fdiv_rn((float)in, (float)out))), in - 1);
+}
+
+__global__ void upsample_nearest_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int B, int H, int W, int C,
+                                        int Ho, int Wo, __nv_bfloat16* __restrict__ y) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int oct = C / 8;
+  long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  long long total = (long long)B * Ho * Wo * oct;
+  if (idx >= total) return;
+  const int o = (int)(idx % oct);
+  long long pix = idx / oct;
+  const int wo = (int)(pix % Wo);
+  const int ho = (int)((pix / Wo) % Ho);
+  const int b = (int)(pix / ((long long)Wo * Ho));
+  const int hs = nearest_src(ho, H, Ho), ws = nearest_src(wo, W, Wo);
+  uint4 u = __ldg(reinterpret_cast<const uint4*>(x + (((long long)b * H + hs) * W + ws) * ldx + o * 8));
+  *reinterpret_cast<uint4*>(y + pix * C + o * 8) = u;
+}
+
+// col[(b,ho,wo), tap*C + c] = x[b, 2ho+kh-1, 2wo+kw-1, c] (zero outside): Downsample2D conv 3x3 / stride 2 / pad 1, which
+// gives ceil(H / 2) x ceil(W / 2) outputs; pad 0 (the VAE's, even sides only) gives H / 2 x W / 2
 __global__ void im2col_s2_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int B, int H, int W, int C, int pad,
                                  __nv_bfloat16* __restrict__ col) {
   pdl_wait();
   pdl_launch_dependents();
-  const int oct = C / 8, Ho = H / 2, Wo = W / 2;
+  const int oct = C / 8, Ho = (H + pad) / 2, Wo = (W + pad) / 2;
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long total = (long long)B * Ho * Wo * 9 * oct;
   if (idx >= total) return;
@@ -346,30 +373,37 @@ __global__ void softmax_rows_kernel(const float* __restrict__ S, long long lds, 
   const int lane = threadIdx.x & 31;
   if (r >= rows) return;
   const float* row = S + r * lds;
+  const int cols4 = cols & ~3;            // float4 body; the last cols % 4 columns (odd token counts) one at a time
   float m = -INFINITY;
-  for (int c = lane * 4; c < cols; c += 128) {
+  for (int c = lane * 4; c < cols4; c += 128) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(row + c));
     m = fmaxf(fmaxf(m, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
   }
+  if (cols4 + lane < cols) m = fmaxf(m, __ldg(row + cols4 + lane));
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
   const float mm = m * scale_log2;
   float sum = 0.f;
-  for (int c = lane * 4; c < cols; c += 128) {
+  for (int c = lane * 4; c < cols4; c += 128) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(row + c));
     sum += exp2f(v.x * scale_log2 - mm) + exp2f(v.y * scale_log2 - mm) + exp2f(v.z * scale_log2 - mm) +
            exp2f(v.w * scale_log2 - mm);
   }
+  if (cols4 + lane < cols) sum += exp2f(__ldg(row + cols4 + lane) * scale_log2 - mm);
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
   const float inv = 1.0f / sum;
   __nv_bfloat16* orow = out + r * ldo;
-  for (int c = lane * 4; c < cols; c += 128) {
+  for (int c = lane * 4; c < cols4; c += 128) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(row + c));
     uint2 o;
     o.x = pack16x2<F16>(exp2f(v.x * scale_log2 - mm) * inv, exp2f(v.y * scale_log2 - mm) * inv);
     o.y = pack16x2<F16>(exp2f(v.z * scale_log2 - mm) * inv, exp2f(v.w * scale_log2 - mm) * inv);
     *reinterpret_cast<uint2*>(orow + c) = o;
+  }
+  if (cols4 + lane < cols) {
+    const float e = exp2f(__ldg(row + cols4 + lane) * scale_log2 - mm) * inv;
+    reinterpret_cast<unsigned short*>(orow)[cols4 + lane] = (unsigned short)(pack16x2<F16>(e, 0.f) & 0xffffu);
   }
 }
 
@@ -553,20 +587,27 @@ extern "C" int mos_conv_out(const void* x, int32_t B, int32_t H, int32_t W, int3
   return MOS_OK;
 }
 
-extern "C" int mos_upsample2x(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, void* y,
-                              void* stream) {
-  MOS_CHECK_ARG(x && y && C % 8 == 0 && ldx % 8 == 0, "mos_upsample2x: bad arguments");
-  long long total = (long long)B * 4 * H * W * (C / 8);
-  MOS_CHECK_CUDA(launch_pdl(upsample2x_kernel, dim3(nblk(total, 256)), dim3(256), 0, STREAM(stream), reinterpret_cast<const __nv_bfloat16*>(x), ldx, B, H,
-                                                                  W, C, reinterpret_cast<__nv_bfloat16*>(y)));
+extern "C" int mos_upsample2x(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, void* y, int32_t Ho,
+                              int32_t Wo, void* stream) {
+  MOS_CHECK_ARG(x && y && C % 8 == 0 && ldx % 8 == 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0, "mos_upsample2x: bad arguments");
+  if (Ho == 2 * H && Wo == 2 * W) {
+    long long total = (long long)B * 4 * H * W * (C / 8);
+    MOS_CHECK_CUDA(launch_pdl(upsample2x_kernel, dim3(nblk(total, 256)), dim3(256), 0, STREAM(stream), reinterpret_cast<const __nv_bfloat16*>(x), ldx, B, H,
+                                                                    W, C, reinterpret_cast<__nv_bfloat16*>(y)));
+    return MOS_OK;
+  }
+  long long total = (long long)B * Ho * Wo * (C / 8);
+  MOS_CHECK_CUDA(launch_pdl(upsample_nearest_kernel, dim3(nblk(total, 256)), dim3(256), 0, STREAM(stream),
+                            reinterpret_cast<const __nv_bfloat16*>(x), ldx, B, H, W, C, Ho, Wo,
+                            reinterpret_cast<__nv_bfloat16*>(y)));
   return MOS_OK;
 }
 
 extern "C" int mos_im2col_s2(const void* x, int64_t ldx, int32_t B, int32_t H, int32_t W, int32_t C, int32_t pad, void* col,
                              void* stream) {
-  MOS_CHECK_ARG(x && col && C % 8 == 0 && ldx % 8 == 0 && H % 2 == 0 && W % 2 == 0 && (pad == 0 || pad == 1),
+  MOS_CHECK_ARG(x && col && C % 8 == 0 && ldx % 8 == 0 && H > 0 && W > 0 && (pad == 1 || (pad == 0 && H % 2 == 0 && W % 2 == 0)),
                 "mos_im2col_s2: bad arguments");
-  long long total = (long long)B * (H / 2) * (W / 2) * 9 * (C / 8);
+  long long total = (long long)B * ((H + pad) / 2) * ((W + pad) / 2) * 9 * (C / 8);
   MOS_CHECK_CUDA(launch_pdl(im2col_s2_kernel, dim3(nblk(total, 256)), dim3(256), 0, STREAM(stream), reinterpret_cast<const __nv_bfloat16*>(x), ldx, B, H,
                                                                  W, C, (int)pad, reinterpret_cast<__nv_bfloat16*>(col)));
   return MOS_OK;
@@ -632,8 +673,8 @@ extern "C" int mos_clip_embed_bwd(const int32_t* ids, const void* dx, int64_t ld
 
 extern "C" int mos_softmax_rows(const float* S, int64_t lds, int64_t rows, int32_t cols, float scale, void* out, int64_t ldo,
                                 int32_t act_dtype, void* stream) {
-  MOS_CHECK_ARG(S && out && rows > 0 && cols > 0 && cols % 4 == 0 && lds % 4 == 0 && lds >= cols && ldo % 4 == 0 && ldo >= cols,
-                "mos_softmax_rows: bad arguments (cols, lds, ldo must be multiples of 4)");
+  MOS_CHECK_ARG(S && out && rows > 0 && cols > 0 && lds % 4 == 0 && lds >= cols && ldo % 4 == 0 && ldo >= cols,
+                "mos_softmax_rows: bad arguments (lds, ldo must be multiples of 4)");
   MOS_CHECK_DTYPE(act_dtype, "mos_softmax_rows");
   const int warps = 8;
   MOS_CHECK_CUDA(launch_pdl(act_dtype ? softmax_rows_kernel<true> : softmax_rows_kernel<false>, dim3(nblk(rows, warps)),

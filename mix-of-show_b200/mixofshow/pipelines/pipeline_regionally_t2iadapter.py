@@ -32,6 +32,18 @@ def region_feat_size(height, width, seq_lens):
     return int(height // downscale), int(width // downscale)       # reference :48
 
 
+def check_region_sizes(height, width, levels, vae_scale_factor=8):
+    """Regional sampling recovers each cross-attention level's (h, w) from its token count with `region_feat_size`; at
+    some image sizes (520 x 520: a 33 x 33 level read as 32 x 32) that rule disagrees with the level's true size, where
+    the reference fails inside `rearrange`.  Refuse those sizes up front, before any text encoding or UNet work."""
+    from mos_b200.engine import level_sizes
+    for lvl, (h, w) in enumerate(level_sizes(height // vae_scale_factor, width // vae_scale_factor, levels)):
+        fh, fw = region_feat_size(height, width, h * w)
+        if (fh, fw) != (h, w):
+            raise ValueError(f'regional sampling cannot run at {height} x {width}: UNet level {lvl} is {h} x {w} latent '
+                             f'pixels, but the region rule recovers {fh} x {fw} from its {h * w} tokens')
+
+
 class RegionT2I_AttnProcessor:
     def __init__(self, cross_attention_idx, attention_op=None):
         self.attention_op = attention_op
@@ -191,6 +203,7 @@ class RegionallyT2IAdapterPipeline:
         device = self.device
         do_cfg = guidance_scale > 1.0
         assert self.new_concept_cfg is not None
+        check_region_sizes(height, width, len(self.unet.config.block_out_channels), self.vae_scale_factor)
         prompt_embeds, region_list = self._encode_region_prompt(
             prompt, self.new_concept_cfg, device, num_images_per_prompt, do_cfg, negative_prompt,
             prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds, height=height, width=width,

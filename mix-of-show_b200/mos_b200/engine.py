@@ -50,6 +50,17 @@ def cross_attention_names(block_out=(320, 640, 1280, 1280), layers=2):
     return names
 
 
+def level_sizes(height, width, levels):
+    """latent (h, w) of every UNet level: diffusers' Downsample2D (3x3, stride 2, pad 1) gives ceil(h / 2) x ceil(w / 2),
+    and each up block interpolates back to the size of the level above (forward_upsample_size), so the levels are exact
+    halvings only when the latent sides are multiples of 2^(levels - 1)."""
+    sizes = [(height, width)]
+    for _ in range(levels - 1):
+        h, w = sizes[-1]
+        sizes.append(((h + 1) // 2, (w + 1) // 2))
+    return sizes
+
+
 def geglu_perm(n):
     """Row order of the packed GEGLU projection (n = 2H output rows): for every 160-column output tile, 80 rows of the value
     half followed by the matching 80 rows of the gate half, so that the fused epilogue finds both halves of an output
@@ -84,6 +95,7 @@ class UNetEngine:
         self.lora_alpha = float(lora_alpha)
         self._merge = lora if merge_lora else None
         self.sd = state_dict
+        self.level_hw = level_sizes(height, width, len(block_out))
         self.w = {}
         self._pack_args = {}
         self.bufs = {}
@@ -268,8 +280,8 @@ class UNetEngine:
         h_ch = rev[0]
         k = 0
         for i in range(nb):
-            res_div = 2 ** (nb - 1 - i)
-            M = B * (H // res_div) * (W // res_div)
+            lh, lw = self.level_hw[nb - 1 - i]
+            M = B * lh * lw
             for j in range(self.layers + 1):
                 cs = skip_ch[len(skip_ch) - 1 - k]
                 ch = h_ch if j == 0 else rev[i]
@@ -497,7 +509,8 @@ class UNetEngine:
         height, width = self.region_hw
         downscale = math.sqrt(height * width / N)                       # regional :45
         fh, fw = int(height // downscale), int(width // downscale)      # regional :48
-        assert fh == h and fw == w
+        if (fh, fw) != (h, w):      # RegionallyT2IAdapterPipeline refuses these sizes up front (check_region_sizes)
+            raise ValueError(f'region rule gives {fh} x {fw} for a {h} x {w} level at {height} x {width}')
         outs, boxes = [], []
         for r, (ehs_layers, box) in enumerate(self.regions):
             Kr, Vr = self.rkv[(r, xidx)]                  # step-invariant: projected once per prompt (update_text)
@@ -608,12 +621,13 @@ class UNetEngine:
             if has_attn:
                 slot = self._skip_slot(si)
                 si += 1
-                Mo = B * (h // 2) * (w // 2)
+                ho, wo = self.level_hw[i + 1]
+                Mo = B * ho * wo
                 col = self.buf('im2col', (Mo, 9 * c))
                 ops.im2col_s2(x, col, B=B, H=h, W=w, C=c, ldx=x.stride(0))
                 self.launches += 1
                 self.gemm(col, self.w[f'down_blocks.{i}.downsamplers.0.conv'], slot, M=Mo)
-                h, w = h // 2, w // 2
+                h, w = ho, wo
                 x = slot
         # mid
         c = self.block_out[-1]
@@ -651,10 +665,12 @@ class UNetEngine:
                     self.resnet(f'up_blocks.{i}.resnets.{j}', xin, nxt, h, w, ch + cs, c)
                 k += 1
                 if last_in_block and not final:
-                    up = self.buf('up_x', (B * 4 * h * w, c))
-                    ops.upsample2x(nxt, up, B=B, H=h, W=w, C=c, ldx=nxt.stride(0))
+                    # diffusers' forward_upsample_size: up to the size of the skip this level concatenates
+                    ho, wo = self.level_hw[nb - 2 - i]
+                    up = self.buf('up_x', (B * ho * wo, c))
+                    ops.upsample2x(nxt, up, B=B, H=h, W=w, C=c, ldx=nxt.stride(0), Ho=ho, Wo=wo)
                     self.launches += 1
-                    h, w = 2 * h, 2 * w
+                    h, w = ho, wo
                     dst = self.cat[k][:, :self.cat_ch[k][0]]
                     self.gemm(up, self.w[f'up_blocks.{i}.upsamplers.0.conv'], dst, M=B * h * w, conv=(B, h, w, c))
         # out

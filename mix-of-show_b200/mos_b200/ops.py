@@ -158,10 +158,12 @@ def conv_out(x, w, bias, y, *, B, H, W, C):
     return y
 
 
-def upsample2x(x, y, *, B, H, W, C, ldx=None):
+def upsample2x(x, y, *, B, H, W, C, ldx=None, Ho=None, Wo=None):
+    """nearest upsample to (Ho, Wo), by default (2H, 2W)"""
     check(_lib.lib().mos_upsample2x(ptr(x), ctypes.c_int64(C if ldx is None else ldx), ctypes.c_int32(B),
-                                    ctypes.c_int32(H), ctypes.c_int32(W), ctypes.c_int32(C), ptr(y), _s()),
-          'mos_upsample2x')
+                                    ctypes.c_int32(H), ctypes.c_int32(W), ctypes.c_int32(C), ptr(y),
+                                    ctypes.c_int32(2 * H if Ho is None else Ho), ctypes.c_int32(2 * W if Wo is None else Wo),
+                                    _s()), 'mos_upsample2x')
     return y
 
 

@@ -57,6 +57,11 @@ class TrainEngine(UNetEngine):
         bf16 [B * 77, 800] rounded from the fp32 layer sum `d_ehs_f32` [B * 77, 800]."""
         if where not in UNET_WHERE:
             raise ValueError(f'where: {where!r} is not one of {UNET_WHERE}')
+        # the backward (col2im_s2, upsample2x_bwd) undoes exact halvings only: a level of odd size would be misread
+        f = 2 ** (len(kw.get('block_out', (320, 640, 1280, 1280))) - 1)
+        if height % f or width % f:
+            raise ValueError(f'training needs latent sides that are multiples of {f} (images of multiples of {8 * f} '
+                             f'pixels); got a {height} x {width} latent')
         self.where = where
         self.shared_ehs = bool(shared_ehs)
         self.use_train_graph = bool(kw.pop('use_graph', True))

@@ -189,14 +189,15 @@ class VAEEngine:
         gn = self.buf('at_gn', (M, C))
         self.groupnorm(x, a + '.group_norm', gn, HW=N, C=C, silu=False)
         Nk = _r(N, 160)                                       # keys padded to the GEMM tile (zero rows, masked by softmax)
+        Np = _r(N, 64)               # the P V GEMM's depth: P's columns and V's tokens past N stay zero (odd latent sizes)
         Q = self.buf('at_Q', (B, N, Cp), zero=True)
         K = self.buf('at_K', (B, Nk, Cp), zero=True)
-        Vt = self.buf('at_Vt', (B, Cp, N), zero=True)
-        hseg = dict(seg_ptr=[Q, K, Vt], seg_kind=[MOS_SEG_ROWS, MOS_SEG_ROWS, MOS_SEG_TRANSPOSED], seg_rows_pad=[N, Nk, N],
+        Vt = self.buf('at_Vt', (B, Cp, Np), zero=True)
+        hseg = dict(seg_ptr=[Q, K, Vt], seg_kind=[MOS_SEG_ROWS, MOS_SEG_ROWS, MOS_SEG_TRANSPOSED], seg_rows_pad=[N, Nk, Np],
                     heads=1, head_dim=Cp, dpad=Cp, dv_pad=Cp, tokens_per_batch=N)
         self.gemm(gn, self.w[a + '.qkv'], None, M=M, heads=hseg)
         S = self.buf('at_S', (N, Nk), F32)
-        P = self.buf('at_P', (N, N))
+        P = self.buf('at_P', (N, Np), zero=True)
         O = self.buf('at_O', (M, Cp))
         for b in range(B):
             ops.gemm(Q[b], K[b], S, M=N, out_f32=True)                           # S = Q K^T   [N, Nk] fp32

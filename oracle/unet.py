@@ -198,8 +198,10 @@ class Upsample2D(nn.Module):
         super().__init__()
         self.conv = nn.Conv2d(channels, channels, 3, padding=1)
 
-    def forward(self, x):
-        return self.conv(F.interpolate(x, scale_factor=2.0, mode='nearest'))
+    def forward(self, x, output_size=None):
+        if output_size is None:
+            return self.conv(F.interpolate(x, scale_factor=2.0, mode='nearest'))
+        return self.conv(F.interpolate(x, size=output_size, mode='nearest'))
 
 
 class CrossAttnDownBlock2D(nn.Module):
@@ -263,11 +265,11 @@ class UpBlock2D(nn.Module):
             self.resnets.append(ResnetBlock2D(rin + skip, cout))
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_upsample else None
 
-    def forward(self, x, skips, temb):
+    def forward(self, x, skips, temb, upsample_size=None):
         for resnet in self.resnets:
             x = resnet(torch.cat([x, skips.pop()], dim=1), temb)
         if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
+            x = self.upsamplers[0](x) if upsample_size is None else self.upsamplers[0](x, upsample_size)
         return x
 
 
@@ -283,11 +285,11 @@ class CrossAttnUpBlock2D(nn.Module):
             self.resnets.append(ResnetBlock2D(rin + skip, cout))
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_upsample else None
 
-    def forward(self, x, skips, temb, ehs, kw):
+    def forward(self, x, skips, temb, ehs, kw, upsample_size=None):
         for resnet, attn in zip(self.resnets, self.attentions):
             x = attn(resnet(torch.cat([x, skips.pop()], dim=1), temb), ehs, kw)
         if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
+            x = self.upsamplers[0](x) if upsample_size is None else self.upsamplers[0](x, upsample_size)
         return x
 
 
@@ -373,11 +375,19 @@ class UNet2DConditionModel(nn.Module):
                     outs[-1] = x
                 skips += outs
         x = self.mid_block(x, temb, encoder_hidden_states, cross_attention_kwargs)
-        for blk in self.up_blocks:
+        # diffusers' forward_upsample_size: when a latent side is not a multiple of 2^(number of upsamplers), the
+        # stride-2 downsamplers round up (ceil) and every non-final up block interpolates to the size of the next skip
+        factor = 2 ** (len(self.up_blocks) - 1)
+        forward_upsample_size = any(s % factor != 0 for s in sample.shape[-2:])
+        for i, blk in enumerate(self.up_blocks):
+            final = i == len(self.up_blocks) - 1
+            size = None
+            if forward_upsample_size and not final:
+                size = skips[-len(blk.resnets) - 1].shape[2:]
             if isinstance(blk, CrossAttnUpBlock2D):
-                x = blk(x, skips, temb, encoder_hidden_states, cross_attention_kwargs)
+                x = blk(x, skips, temb, encoder_hidden_states, cross_attention_kwargs, size)
             else:
-                x = blk(x, skips, temb)
+                x = blk(x, skips, temb, size)
         x = self.conv_out(self.conv_act(self.conv_norm_out(x)))
         return SimpleNamespace(sample=x)
 

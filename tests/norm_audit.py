@@ -19,8 +19,8 @@ Element bound (a).  u = 2^-24 (fp32), u16 = 2^-8 (bf16) / 2^-11 (fp16), t16 the 
 (gemm_audit.TINY_OUT); every 16-bit output adds u16 |ref| + t16 to the fp32 error e below: |got - ref| <= u16 |ref| +
 (1 + u16) e + t16.  An fp32 sum of n terms in any order errs by at most (n - 1) u sum |terms| (plus second-order terms,
 covered by using n + 8).
-- upsample2x, im2col_s2 (taps and zero pads), clip_embed's pad columns [C, ld), t_out of cfg_dpmpp_step and
-  region_combine where at most one region covers a pixel: bit-exact (e = 0, no output rounding).
+- upsample2x (at 2x and at any other output size), im2col_s2 (taps and zero pads), clip_embed's pad columns [C, ld),
+  t_out of cfg_dpmpp_step and region_combine where at most one region covers a pixel: bit-exact (e = 0, no output rounding).
 - add_rows, clip_embed: one fp32 add, e = u |a + b|.
 - upsample2x_bwd, col2im_s2 (with `add`): sums of at most 4 (5) terms, e = 5u sum |terms|.
 - conv_out (9C products per output, lane sums, the butterfly and the bias) and conv_out_bwd (9 Cout products):
@@ -113,7 +113,7 @@ _ARGS = {
                           'ldy', 'act_dtype'),
     'mos_layernorm_fwd': ('x', 'ldx', 'M', 'C', 'gamma', 'beta', 'eps', 'y', 'ldy', 'act_dtype'),
     'mos_conv_out': ('x', 'B', 'H', 'W', 'C', 'w', 'bias', 'Cout', 'y', 'act_dtype'),
-    'mos_upsample2x': ('x', 'ldx', 'B', 'H', 'W', 'C', 'y'),
+    'mos_upsample2x': ('x', 'ldx', 'B', 'H', 'W', 'C', 'y', 'Ho', 'Wo'),
     'mos_im2col_s2': ('x', 'ldx', 'B', 'H', 'W', 'C', 'pad', 'col'),
     'mos_add_rows': ('x', 'ldx', 'r', 'ldr', 'M', 'C', 'act_dtype'),
     'mos_clip_embed': ('ids', 'tok', 'pos', 'M', 'T', 'C', 'vocab', 'x', 'ld'),
@@ -236,6 +236,8 @@ def norm_path(rec):
         return '|'.join(key + ['silu'] * bool(a['silu']))
     if e == 'mos_layernorm_fwd':
         return f"ln|{dt}|C={a['C']}" + ('|mtail' if a['M'] % 8 else '')
+    if e == 'mos_upsample2x':
+        return 'upsample2x' + ('' if (a['Ho'], a['Wo']) == (2 * a['H'], 2 * a['W']) else '|sized')
     if e == 'mos_im2col_s2':
         return f"im2col|pad={a['pad']}"
     if e == 'mos_region_combine':
@@ -323,13 +325,13 @@ def record(entry, a, S, call=None):
         win('bias', F32, (a['Cout'],), (1,))
         target('y', F32, (B, a['Cout'], H, W), (a['Cout'] * H * W, H * W, W, 1))
     elif entry == 'mos_upsample2x':
-        B, H, W, C = a['B'], a['H'], a['W'], a['C']
+        B, H, W, C, Ho, Wo = a['B'], a['H'], a['W'], a['C'], a['Ho'], a['Wo']
         win('x', BF, (B, H, W, C), (H * W * a['ldx'], W * a['ldx'], a['ldx'], 1), ld=a['ldx'])
-        target('y', BF, (B, 2 * H, 2 * W, C), (4 * H * W * C, 2 * W * C, C, 1), ld=C)
+        target('y', BF, (B, Ho, Wo, C), (Ho * Wo * C, Wo * C, C, 1), ld=C)
     elif entry == 'mos_im2col_s2':
         B, H, W, C = a['B'], a['H'], a['W'], a['C']
         win('x', BF, (B, H, W, C), (H * W * a['ldx'], W * a['ldx'], a['ldx'], 1), ld=a['ldx'])
-        Ho, Wo = H // 2, W // 2
+        Ho, Wo = (H + a['pad']) // 2, (W + a['pad']) // 2                 # pad 1: ceil (any side); pad 0: even sides
         target('col', BF, (B, Ho, Wo, 9, C), (Ho * Wo * 9 * C, Wo * 9 * C, 9 * C, C, 1), ld=9 * C)
     elif entry == 'mos_add_rows':
         dt = _dt(a)
@@ -623,6 +625,16 @@ def _norm_ref(rec, x, dims, silu):
     return y, 1.1 * e_z + y.abs() * ((1 - s) * _e_exp(z) + 2 * U32)
 
 
+def nearest_src(dst, n_in, n_out):
+    """source index of output row / column `dst` of a nearest resize from n_in to n_out: PyTorch's upsample_nearest2d with
+    an explicit size, min(floor(dst * (float)(n_in / n_out)), n_in - 1) in fp32, and dst >> 1 at exactly 2x"""
+    if n_out == 2 * n_in:
+        return dst >> 1
+    scale = (torch.tensor(n_in, dtype=F32) / torch.tensor(n_out, dtype=F32)).item()      # fp32 quotient
+    prod = (torch.tensor(dst, dtype=F32) * torch.tensor(scale, dtype=F32)).item()     # fp32 product
+    return min(math.floor(prod), n_in - 1)
+
+
 def reference(rec):
     """float64 reference of every output target: {name: (ref, fp32 error bound)}; bound None: bit-exact"""
     e, a, x = rec['op'], rec['abi'], rec['in']
@@ -637,7 +649,10 @@ def reference(rec):
         mag = torch.nn.functional.conv2d(X.abs(), W.abs(), x['bias'].double().abs(), padding=1)
         return {'y': (y, (9 * a['C'] + 8) * U32 * mag)}
     if e == 'mos_upsample2x':
-        return {'y': (x['x'].repeat_interleave(2, 1).repeat_interleave(2, 2), None)}
+        X = x['x']
+        rows = torch.tensor([nearest_src(i, a['H'], a['Ho']) for i in range(a['Ho'])], device=X.device)
+        cols = torch.tensor([nearest_src(j, a['W'], a['Wo']) for j in range(a['Wo'])], device=X.device)
+        return {'y': (X[:, rows][:, :, cols], None)}
     if e == 'mos_im2col_s2':
         p = a['pad']
         X = torch.nn.functional.pad(x['x'], (0, 0, p, 2 - p, p, 2 - p))    # rows -p .. H + 1 - p

@@ -109,7 +109,9 @@ def down_fwd(self, x):
     return C.rs(lin(self.conv, x))
 
 
-def up_fwd(self, x):
+def up_fwd(self, x, output_size=None):
+    if output_size is not None:
+        return C.rs(lin(self.conv, F.interpolate(x, size=output_size, mode='nearest')))
     return C.rs(lin(self.conv, F.interpolate(x, scale_factor=2.0, mode='nearest')))
 
 
