@@ -22,6 +22,7 @@ import os
 import torch
 
 from mos_b200 import ops
+from mos_b200.dp import init_distributed
 
 F32 = torch.float32
 
@@ -911,25 +912,6 @@ def parse_args(argv=None):
     parser.add_argument('--optimize_unet_iters', default=50, type=int)
     parser.add_argument('--optimize_textenc_iters', default=500, type=int)
     return parser.parse_args(argv)
-
-
-def init_distributed():
-    """torchrun environment (WORLD_SIZE / RANK / LOCAL_RANK, as train_edlora.py reads it) -> (rank, world, device).  Ranks
-    take device LOCAL_RANK modulo the visible devices: NCCL when every rank has a GPU of its own, gloo when ranks share
-    one (more ranks on this node, LOCAL_WORLD_SIZE, than visible devices).  Without WORLD_SIZE nothing is initialised:
-    (0, 1, 'cuda')."""
-    import torch.distributed as dist
-    world = int(os.environ.get('WORLD_SIZE', '1'))
-    if world == 1:
-        return 0, 1, 'cuda'
-    n_dev = torch.cuda.device_count()
-    device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0')) % n_dev}"
-    torch.cuda.set_device(device)
-    if int(os.environ.get('LOCAL_WORLD_SIZE', world)) <= n_dev:
-        dist.init_process_group('nccl', device_id=torch.device(device))
-    else:
-        dist.init_process_group('gloo')
-    return dist.get_rank(), world, device
 
 
 def main(argv=None):

@@ -6,6 +6,8 @@ pass per prompt, one [B, 77, 768] embedding for every cross-attention layer (the
 
 The denoise loop (reference :271-301) runs on the GPU engine: per step one captured UNet graph (CFG batch 2) and
 ONE fused kernel for CFG combine + DPM-Solver++(2M) update + re-duplication of the latents (`mos_cfg_dpmpp_step`).
+With `cfg_group` two ranks share one call: each runs one CFG half at batch 1 and they exchange eps once per step
+(`denoise_latents`, shared with the regional pipeline).
 Prompt encoding and image decoding run on the GPU CLIP / VAE engines (mixofshow/models/clip_b200.py, vae_b200.py) when
 `from_pretrained` finds `text_encoder/` and `vae/`; without them pass `prompt_embeds` and request `output_type='latent'`.
 """
@@ -16,7 +18,7 @@ import torch
 
 from mixofshow.models.edlora import (revise_edlora_unet_attention_controller_forward,
                                      revise_edlora_unet_attention_forward)
-from mos_b200 import ops
+from mos_b200 import dp, ops
 from mos_b200.scheduler import DPMSolverPP2M
 
 
@@ -42,6 +44,66 @@ def bind_concept_prompt(prompts, new_concept_cfg):
                          for p, new_name in zip(per_layer, new_token_cfg['concept_token_names'])]
         new_prompts.extend(per_layer)
     return new_prompts
+
+
+def denoise_latents(unet, scheduler, latents, guidance_scale, prompt_embeds, cross_attention_kwargs=None,
+                    adapter_state=None, controller=None, callback=None, callback_steps=1, cfg_group=None):
+    """The denoise loop of both pipelines (reference pipeline_edlora.py:271-301, pipeline_regionally_t2iadapter.py:548-580),
+    over `scheduler.timesteps`; updates and returns `latents` [n, 4, h, w] (already scaled by init_noise_sigma).
+    `prompt_embeds` and the region embeddings of `cross_attention_kwargs['region_list']` hold the CFG halves uncond | cond
+    along the batch ([2n, ...] with guidance > 1); `adapter_state` holds the adapter residuals once ([n, C, h', w']).
+
+    One prepared session: weights verified / packed and the step-invariant inputs uploaded ONCE; a step is then one graph
+    replay + one fused CFG / DPM-Solver++ kernel, with no host synchronisation inside the loop.
+
+    With `cfg_group` (two ranks, dp.check_cfg_group) group rank i runs only half i (0 = uncond, 1 = cond) as a batch-n
+    session, and each step all-gathers the two eps halves into the [2n] layout the fused step reads (dp.CFGExchange).
+    Both ranks then run the same fused step on the same inputs, so they hold the same latents bit for bit; the initial
+    latents are those of group rank 0."""
+    do_cfg = guidance_scale > 1.0
+    timesteps = [int(t) for t in scheduler.timesteps]
+    n, _, h, w = latents.shape
+    device = latents.device
+    exchange = None
+    if cfg_group is None:
+        nb = 2 * n if do_cfg else n
+        if do_cfg and adapter_state is not None:
+            adapter_state = [torch.cat([v] * 2, dim=0) for v in adapter_state]
+    else:
+        nb = n
+        exchange = dp.CFGExchange(cfg_group, tuple(latents.shape), device)
+        exchange.broadcast(latents)
+        half = slice(exchange.half * n, (exchange.half + 1) * n)
+        prompt_embeds = prompt_embeds[half]
+        if cross_attention_kwargs and 'region_list' in cross_attention_kwargs:
+            cross_attention_kwargs = dict(cross_attention_kwargs, region_list=[
+                (emb[half], box) for emb, box in cross_attention_kwargs['region_list']])
+    x0_prev = torch.zeros_like(latents)
+    sess = unet.session(nb, h, w, device, prompt_embeds, cross_attention_kwargs, adapter_state)
+    unet_in = sess.latents_in
+    unet_in.copy_(torch.cat([latents] * 2) if nb > n else latents)
+    sess.t_in.fill_(float(timesteps[0]))
+    for i, t in enumerate(timesteps):
+        noise_pred = sess.step()
+        t_next = float(timesteps[i + 1]) if i + 1 < len(timesteps) else 0.0
+        coef = scheduler.coefficients(i)
+        if exchange is None:
+            # CFG combine + scheduler.step + cat([latents]*2) + next timestep, one kernel (reference :285-290, :273)
+            ops.cfg_dpmpp_step(noise_pred, latents, x0_prev, unet_in.view(-1), cfg=do_cfg,
+                               guidance=float(guidance_scale), coef=coef, t_out=sess.t_in, t_next=t_next)
+        else:
+            # the batch-n session takes one copy of the next input, the kernel would write two
+            ops.cfg_dpmpp_step(exchange.all_gather(noise_pred), latents, x0_prev, None, cfg=True,
+                               guidance=float(guidance_scale), coef=coef, t_out=sess.t_in, t_next=t_next)
+            unet_in.copy_(latents)
+        if controller is not None and hasattr(controller, 'step_callback'):
+            new_latents = controller.step_callback(latents)
+            if new_latents is not latents:      # a controller may return edited latents (reference :293-295)
+                latents.copy_(new_latents.to(latents.dtype))
+                unet_in.copy_(torch.cat([latents] * 2) if do_cfg else latents)
+        if callback is not None and i % callback_steps == 0:
+            callback(i, t, latents)
+    return latents
 
 
 class _GPUPipeline:
@@ -104,12 +166,10 @@ class _GPUPipeline:
         return negative_prompt
 
     def _denoise(self, prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator, latents,
-                 output_type, return_dict, callback, callback_steps, cross_attention_kwargs):
+                 output_type, return_dict, callback, callback_steps, cross_attention_kwargs, cfg_group):
         """reference :262-322 from the timesteps to the decoded images; `prompt_embeds` carries the CFG halves"""
         device = self.device
-        do_cfg = guidance_scale > 1.0
         self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = [int(t) for t in self.scheduler.timesteps]
         h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
         shape = (batch_size, self.unet.in_channels, h, w)
         if latents is None:
@@ -118,29 +178,9 @@ class _GPUPipeline:
         latents = (latents.to(device, torch.float32) * self.scheduler.init_noise_sigma).contiguous()
         assert tuple(latents.shape) == shape, f'latents shape {tuple(latents.shape)} != {shape}'
 
-        controller = getattr(self, 'controller', None)
-        x0_prev = torch.zeros_like(latents)
-        nb = 2 * batch_size if do_cfg else batch_size
-        # one prepared session: weights verified / packed and the step-invariant inputs uploaded ONCE; a step is then one
-        # graph replay + one fused kernel, with no host synchronisation inside the loop (reference loop :271-301)
-        sess = self.unet.session(nb, h, w, device, prompt_embeds, cross_attention_kwargs)
-        unet_in = sess.latents_in
-        unet_in.copy_(torch.cat([latents] * 2) if do_cfg else latents)
-        sess.t_in.fill_(float(timesteps[0]))
-        for i, t in enumerate(timesteps):
-            noise_pred = sess.step()
-            # CFG combine + scheduler.step + cat([latents]*2) + next timestep, one kernel (reference :285-290, :273)
-            t_next = float(timesteps[i + 1]) if i + 1 < len(timesteps) else 0.0
-            ops.cfg_dpmpp_step(noise_pred, latents, x0_prev, unet_in.view(-1), cfg=do_cfg,
-                               guidance=float(guidance_scale), coef=self.scheduler.coefficients(i), t_out=sess.t_in,
-                               t_next=t_next)
-            if controller is not None and hasattr(controller, 'step_callback'):
-                new_latents = controller.step_callback(latents)
-                if new_latents is not latents:      # a controller may return edited latents (reference :293-295)
-                    latents.copy_(new_latents.to(latents.dtype))
-                    unet_in.copy_(torch.cat([latents] * 2) if do_cfg else latents)
-            if callback is not None and i % callback_steps == 0:
-                callback(i, t, latents)
+        denoise_latents(self.unet, self.scheduler, latents, guidance_scale, prompt_embeds, cross_attention_kwargs,
+                        controller=getattr(self, 'controller', None), callback=callback, callback_steps=callback_steps,
+                        cfg_group=cfg_group)
         if output_type == 'latent':
             image = latents
         else:
@@ -214,7 +254,11 @@ class EDLoRAPipeline(_GPUPipeline):
                  negative_prompt=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
                  latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
                  negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = 'pil',
-                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None):
+                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None,
+                 cfg_group=None):
+        """`cfg_group`: a torch.distributed group of two ranks that sample this one call together, rank 0 the uncond
+        and rank 1 the cond half of every UNet call (`denoise_latents`); both return the same images."""
+        dp.check_cfg_group(cfg_group, guidance_scale, getattr(self, 'controller', None))
         height = height or self.unet.config.sample_size * self.vae_scale_factor
         width = width or self.unet.config.sample_size * self.vae_scale_factor
         if height % 8 != 0 or width % 8 != 0:
@@ -227,7 +271,8 @@ class EDLoRAPipeline(_GPUPipeline):
                                             negative_prompt, prompt_embeds=prompt_embeds,
                                             negative_prompt_embeds=negative_prompt_embeds)
         return self._denoise(prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator,
-                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs)
+                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs,
+                             cfg_group)
 
 
 class StableDiffusionPipeline(_GPUPipeline):
@@ -276,7 +321,11 @@ class StableDiffusionPipeline(_GPUPipeline):
                  negative_prompt=None, num_images_per_prompt: Optional[int] = 1, eta: float = 0.0, generator=None,
                  latents: Optional[torch.Tensor] = None, prompt_embeds: Optional[torch.Tensor] = None,
                  negative_prompt_embeds: Optional[torch.Tensor] = None, output_type: Optional[str] = 'pil',
-                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None):
+                 return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None,
+                 cfg_group=None):
+        """`cfg_group`: a torch.distributed group of two ranks that sample this one call together, rank 0 the uncond
+        and rank 1 the cond half of every UNet call (`denoise_latents`); both return the same images."""
+        dp.check_cfg_group(cfg_group, guidance_scale, getattr(self, 'controller', None))
         height = height or self.unet.config.sample_size * self.vae_scale_factor
         width = width or self.unet.config.sample_size * self.vae_scale_factor
         if height % 8 != 0 or width % 8 != 0:
@@ -286,4 +335,5 @@ class StableDiffusionPipeline(_GPUPipeline):
                                             negative_prompt, prompt_embeds=prompt_embeds,
                                             negative_prompt_embeds=negative_prompt_embeds)
         return self._denoise(prompt_embeds, batch_size, height, width, num_inference_steps, guidance_scale, generator,
-                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs)
+                             latents, output_type, return_dict, callback, callback_steps, cross_attention_kwargs,
+                             cfg_group)

@@ -14,9 +14,9 @@ from types import SimpleNamespace
 
 import torch
 
-from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt
+from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt, denoise_latents
+from mos_b200 import dp
 from mos_b200 import functional as Fm
-from mos_b200 import ops
 from mos_b200.scheduler import DPMSolverPP2M
 
 
@@ -196,10 +196,13 @@ class RegionallyT2IAdapterPipeline:
                  guidance_scale: float = 7.5, negative_prompt=None, num_images_per_prompt=1, eta: float = 0.0,
                  generator=None, latents=None, prompt_embeds=None, negative_prompt_embeds=None, output_type='pil',
                  return_dict: bool = True, callback=None, callback_steps: int = 1, cross_attention_kwargs=None,
-                 region_list=None, keypose_adapter_state=None, sketch_adapter_state=None):
+                 region_list=None, keypose_adapter_state=None, sketch_adapter_state=None, cfg_group=None):
         """Extra (GPU path) arguments: `region_list` = [(region_embeds [2,16,77,768], box fractions)] and
         `*_adapter_state` = precomputed T2I-Adapter feature maps (4 NCHW tensors), for use without CLIP / adapters; a
-        state takes the place of the adapter run on the matching `*_adapter_input`."""
+        state takes the place of the adapter run on the matching `*_adapter_input`.  `cfg_group`: a torch.distributed
+        group of two ranks that sample this one image together, rank 0 the uncond and rank 1 the cond half of every UNet
+        call (pipeline_edlora.denoise_latents); both run the adapters and return the same image."""
+        dp.check_cfg_group(cfg_group, guidance_scale)
         device = self.device
         do_cfg = guidance_scale > 1.0
         assert self.new_concept_cfg is not None
@@ -209,7 +212,6 @@ class RegionallyT2IAdapterPipeline:
             prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds, height=height, width=width,
             region_list=region_list)
         self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = [int(t) for t in self.scheduler.timesteps]
         h, w = height // self.vae_scale_factor, width // self.vae_scale_factor
         shape = (1, self.unet.config.in_channels, h, w)
         if latents is None:
@@ -233,25 +235,13 @@ class RegionallyT2IAdapterPipeline:
                 if sketch_adapter_state is not None:
                     fs = _spatial_weight(sketch_adapter_state[i], sketch_adaptor_weight, region_sketch_adaptor_weight,
                                          height, width)
-                v = fk + fs
-                adapter_state.append(torch.cat([v] * 2, dim=0) if do_cfg else v)
+                adapter_state.append(fk + fs)
 
-        x0_prev = torch.zeros_like(latents)
+        # region embeddings / boxes and the adapter residuals are step-invariant and uploaded once (reference loop
+        # :548-580)
         kwargs = {'region_list': region_list, 'height': height, 'width': width}
-        # one prepared session (reference loop :548-580): region embeddings / boxes and the adapter residuals are
-        # step-invariant and uploaded once; a step is one graph replay + one fused CFG / DPM-Solver++ kernel
-        sess = self.unet.session(2 if do_cfg else 1, h, w, device, prompt_embeds, kwargs, adapter_state)
-        unet_in = sess.latents_in
-        unet_in.copy_(torch.cat([latents] * 2) if do_cfg else latents)
-        sess.t_in.fill_(float(timesteps[0]))
-        for i, t in enumerate(timesteps):
-            noise_pred = sess.step()
-            t_next = float(timesteps[i + 1]) if i + 1 < len(timesteps) else 0.0
-            ops.cfg_dpmpp_step(noise_pred, latents, x0_prev, unet_in.view(-1), cfg=do_cfg,
-                               guidance=float(guidance_scale), coef=self.scheduler.coefficients(i), t_out=sess.t_in,
-                               t_next=t_next)
-            if callback is not None and i % callback_steps == 0:
-                callback(i, t, latents)
+        denoise_latents(self.unet, self.scheduler, latents, guidance_scale, prompt_embeds, kwargs, adapter_state,
+                        callback=callback, callback_steps=callback_steps, cfg_group=cfg_group)
         if output_type == 'latent':
             image = latents
         else:

@@ -5,11 +5,32 @@ flat fp32 buffer [concept rows | text-encoder LoRA | UNet LoRA | 2 logged scalar
 (NCCL over NVLink on the GPU box, gloo in the CPU tests); the arithmetic after it is mos_flat_adamw_step.
 Gradient fusion shards by layer instead (gradient_fusion.fusion_plan): every rank solves its own layers and the solved
 weights are broadcast by their owners (all_ranks_ok, broadcast_owned).
+Sampling one image splits classifier-free guidance instead: two ranks each run one half (uncond | cond) of every UNet
+call and exchange the two eps halves once per step (check_cfg_group, CFGExchange).
 """
 import math
+import os
 
 import torch
 import torch.distributed as dist
+
+
+def init_distributed():
+    """torchrun environment (WORLD_SIZE / RANK / LOCAL_RANK, as train_edlora.py reads it) -> (rank, world, device).  Ranks
+    take device LOCAL_RANK modulo the visible devices: NCCL when every rank has a GPU of its own, gloo when ranks share
+    one (more ranks on this node, LOCAL_WORLD_SIZE, than visible devices).  Without WORLD_SIZE nothing is initialised:
+    (0, 1, 'cuda')."""
+    world = int(os.environ.get('WORLD_SIZE', '1'))
+    if world == 1:
+        return 0, 1, 'cuda'
+    n_dev = torch.cuda.device_count()
+    device = f"cuda:{int(os.environ.get('LOCAL_RANK', '0')) % n_dev}"
+    torch.cuda.set_device(device)
+    if int(os.environ.get('LOCAL_WORLD_SIZE', world)) <= n_dev:
+        dist.init_process_group('nccl', device_id=torch.device(device))
+    else:
+        dist.init_process_group('gloo')
+    return dist.get_rank(), world, device
 
 
 class FlatTrainState:
@@ -120,6 +141,67 @@ def broadcast_owned(owned, plan, shapes, device):
         for n, part in zip(names, buf.split(sizes)):
             out[n] = part.view(shapes[n])
     return out
+
+
+def check_cfg_group(cfg_group, guidance_scale, controller=None):
+    """Refusals of a CFG-split sampling call (`cfg_group` of the pipelines), made before any text encoding.  They depend
+    only on the call's arguments, so both ranks raise and neither is left waiting in the first exchange."""
+    if cfg_group is None:
+        return
+    if not dist.is_initialized():
+        raise ValueError('cfg_group needs an initialised torch.distributed process group')
+    if dist.get_world_size(cfg_group) != 2 or dist.get_rank(cfg_group) not in (0, 1):
+        raise ValueError(f'cfg_group must be a group of exactly two ranks that includes this one (the uncond and the '
+                         f'cond half); got a group of {dist.get_world_size(cfg_group)}')
+    if guidance_scale <= 1.0:
+        raise ValueError(f'cfg_group splits classifier-free guidance, which guidance_scale {guidance_scale} <= 1 '
+                         f'turns off: there is only one half to run')
+    if controller is not None:
+        raise ValueError('cfg_group cannot run with an attention controller: it edits the cond half of the '
+                         'cross-attention maps, and that half runs on one rank only')
+
+
+class CFGExchange:
+    """The one collective of a CFG-split denoise step: group rank 0 runs the uncond half, rank 1 the cond half, and each
+    step all-gathers the two eps halves ([n, 4, h, w] each) into one [2n, 4, h, w] buffer in group-rank order, the
+    layout `mos_cfg_dpmpp_step` reads with cfg=1.  Under NCCL the gather is ordered on the current stream between the
+    UNet replay and the fused step, with no host synchronisation; under gloo (ranks sharing one GPU) it is staged
+    through host memory."""
+
+    def __init__(self, group, half_shape, device):
+        self.group = group
+        self.half = dist.get_rank(group)
+        n, *rest = half_shape
+        self.out = torch.empty(2 * n, *rest, device=device)
+        self.host = dist.get_backend(group) == 'gloo'
+        if self.host:
+            self.host_in = torch.empty(half_shape)
+            self.host_out = torch.empty(2 * n, *rest)
+
+    @property
+    def bytes_per_step(self):
+        """bytes that cross the wire per step: both eps halves"""
+        return self.out.numel() * self.out.element_size()
+
+    def all_gather(self, eps_half):
+        if self.host:
+            self.host_in.copy_(eps_half)
+            dist.all_gather_into_tensor(self.host_out, self.host_in, group=self.group)
+            self.out.copy_(self.host_out)
+        else:
+            dist.all_gather_into_tensor(self.out, eps_half.contiguous(), group=self.group)
+        return self.out
+
+    def broadcast(self, t):
+        """`t` of group rank 0 on both ranks (the initial latents, so both start the loop from the same noise)"""
+        src = dist.get_global_rank(self.group, 0)
+        if self.host:
+            h = t.cpu()
+            dist.broadcast(h, src=src, group=self.group)
+            t.copy_(h)
+        else:
+            dist.broadcast(t, src=src, group=self.group)
+        return t
 
 
 def optimizer_step(state, grad_scale, norm_out=None):

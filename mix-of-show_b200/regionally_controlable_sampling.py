@@ -114,11 +114,28 @@ def load_conditions(args):
 
 
 def main(argv=None):
+    """`python regionally_controlable_sampling.py ...`, or `torchrun --nproc_per_node 2 ...`: the two ranks sample the one
+    image together, each running one classifier-free-guidance half (RegionallyT2IAdapterPipeline's `cfg_group`), and
+    rank 0 alone writes the outputs."""
+    import torch.distributed as dist
+    from mos_b200 import dp
     args = parse_args(argv)
     conds = load_conditions(args)
-    device = torch.device('cuda')
+    world = int(os.environ.get('WORLD_SIZE', '1'))
+    if world not in (1, 2):
+        raise ValueError(f'regional sampling runs on 1 process, or on 2 under torchrun (one classifier-free-guidance '
+                         f'half each); got WORLD_SIZE={world}')
+    rank, world, device = dp.init_distributed()
+    try:
+        return _sample(args, conds, rank, torch.device(device), dist.group.WORLD if world == 2 else None)
+    finally:
+        if world > 1:
+            dist.destroy_process_group()
+
+
+def _sample(args, conds, rank, device, cfg_group):
     pipe = build_model(args.pretrained_model, device)
-    kwargs = {'height': args.height, 'width': args.width, 'output_type': 'latent'}
+    kwargs = {'height': args.height, 'width': args.width, 'output_type': 'latent', 'cfg_group': cfg_group}
     for kind in ('sketch', 'keypose'):
         path = getattr(args, f'{kind}_adapter_state')
         if path is not None:
@@ -133,7 +150,7 @@ def main(argv=None):
     latents = sample_image(pipe, input_prompt=input_prompt, input_neg_prompt=[args.negative_prompt],
                            generator=torch.Generator('cpu').manual_seed(args.seed),
                            num_inference_steps=args.num_inference_steps, **kwargs)
-    if args.save_dir is not None:
+    if args.save_dir is not None and rank == 0:
         os.makedirs(args.save_dir, exist_ok=True)
         out = os.path.join(args.save_dir, f'latents---{args.seed}{"---" + args.suffix if args.suffix else ""}.pt')
         # condition options that were not given are left out, so an unconditioned run records what it always did
