@@ -821,9 +821,10 @@ def _sharded(stage, shapes, iters, rank, world, device, args, kw):
 def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, pretrained_model_path, save_path, suffix,
                      device='cuda', tokenizer=None, log=print):
     """gradient_fusion.py:750-813 on the GPU path.  `pretrained_model_path`: diffusers-layout directory (unet/,
-    text_encoder/, tokenizer/); the fused UNet / text encoder and new_concept_cfg.json are written to
-    `{save_path}/combined_model_{suffix}` together with the tokenizer that carries the added `<new{k}>` tokens (the VAE /
-    scheduler folders of the base model are untouched by the fusion and are not copied here).
+    text_encoder/, tokenizer/[, vae/, scheduler/]); the fused UNet / text encoder and new_concept_cfg.json are written to
+    `{save_path}/combined_model_{suffix}` together with the tokenizer that carries the added `<new{k}>` tokens, and the
+    base model's vae/ and scheduler/ folders, which the fusion does not change, are copied there byte for byte when they
+    exist: the directory loads as a whole pipeline (EDLoRAPipeline.from_pretrained, regionally_controlable_sampling.py).
     With torch.distributed initialised, the layer solves of every stage are sharded over the ranks (fusion_plan): each rank
     replays the recording, solves its own layers and receives the others' (_sharded); the fused model is the one of a
     single process, bit for bit.  Only rank 0 writes it, and every rank returns once it is written."""
@@ -896,7 +897,8 @@ def compose_concepts(concept_cfg, optimize_textenc_iters, optimize_unet_iters, p
         unet.load_state_dict(sd)
     out_dir = os.path.join(save_path, f'combined_model_{suffix}')
     if rank == 0:
-        model_io.save_combined_model(out_dir, unet, text_encoder, new_concept_cfg, tokenizer=tokenizer)
+        model_io.save_combined_model(out_dir, unet, text_encoder, new_concept_cfg, tokenizer=tokenizer,
+                                     base_model=pretrained_model_path)
     if world > 1:
         dist.barrier()
     return out_dir, new_concept_cfg

@@ -31,6 +31,16 @@ def numpy_to_pil(images):
     return [Image.fromarray(im) for im in (images * 255).round().astype('uint8')]
 
 
+def decode_latents(vae, latents, output_type='pil'):
+    """reference :303-313: `vae.decode(latents / 0.18215)` on the GPU VAE, mapped to [0, 1] -> [N, H, W, 3] floats, or
+    PIL images when `output_type` is 'pil'"""
+    if vae is None:
+        raise ValueError("no VAE supplied: use output_type='latent'")
+    image = vae.decode(latents / 0.18215).sample
+    image = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).float().numpy()
+    return numpy_to_pil(image) if output_type == 'pil' else image
+
+
 def bind_concept_prompt(prompts, new_concept_cfg):
     """Each prompt becomes 16 layer-specific prompts; `concept_name` -> `concept_token_names[layer]`
     (reference :18-29). Output order: prompt-major, layer fastest."""
@@ -181,15 +191,7 @@ class _GPUPipeline:
         denoise_latents(self.unet, self.scheduler, latents, guidance_scale, prompt_embeds, cross_attention_kwargs,
                         controller=getattr(self, 'controller', None), callback=callback, callback_steps=callback_steps,
                         cfg_group=cfg_group)
-        if output_type == 'latent':
-            image = latents
-        else:
-            if self.vae is None:
-                raise ValueError("no VAE supplied: use output_type='latent'")
-            image = self.vae.decode(latents / 0.18215).sample
-            image = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).float().numpy()
-            if output_type == 'pil':
-                image = numpy_to_pil(image)
+        image = latents if output_type == 'latent' else decode_latents(self.vae, latents, output_type)
         if not return_dict:
             return (image)
         return SimpleNamespace(images=image, nsfw_content_detected=None)

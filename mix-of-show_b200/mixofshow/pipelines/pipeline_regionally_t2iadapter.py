@@ -14,7 +14,7 @@ from types import SimpleNamespace
 
 import torch
 
-from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt, denoise_latents
+from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt, decode_latents, denoise_latents
 from mos_b200 import dp
 from mos_b200 import functional as Fm
 from mos_b200.scheduler import DPMSolverPP2M
@@ -242,16 +242,7 @@ class RegionallyT2IAdapterPipeline:
         kwargs = {'region_list': region_list, 'height': height, 'width': width}
         denoise_latents(self.unet, self.scheduler, latents, guidance_scale, prompt_embeds, kwargs, adapter_state,
                         callback=callback, callback_steps=callback_steps, cfg_group=cfg_group)
-        if output_type == 'latent':
-            image = latents
-        else:
-            if self.vae is None:
-                raise ValueError("no VAE supplied: use output_type='latent'")
-            image = self.vae.decode(latents / 0.18215).sample
-            image = (image / 2 + 0.5).clamp(0, 1).cpu().permute(0, 2, 3, 1).float().numpy()
-            if output_type == 'pil':
-                from mixofshow.pipelines.pipeline_edlora import numpy_to_pil
-                image = numpy_to_pil(image)
+        image = latents if output_type == 'latent' else decode_latents(self.vae, latents, output_type)
         if not return_dict:
             return (image, None)
         return SimpleNamespace(images=image, nsfw_content_detected=None)

@@ -9,8 +9,9 @@
     adapters `regionally_controlable_sampling.py:62-63` loads.
 
 `load_unet` / `load_text_encoder` build this repo's GPU containers from such a directory; `save_combined_model` writes
-one.  diffusers itself is not a dependency: the UNet `config.json` keys are the SD1.5 ones (diffusers 0.19.3), and any
-option this path does not implement is rejected loudly instead of being ignored."""
+one, with the base model's `vae/` and `scheduler/` folders copied beside the fused weights.  diffusers itself is not a
+dependency: the UNet `config.json` keys are the SD1.5 ones (diffusers 0.19.3), and any option this path does not
+implement is rejected loudly instead of being ignored."""
 import json
 import os
 
@@ -210,17 +211,25 @@ def save_t2i_adapter(adapter, model_dir, subfolder=None, safe_serialization=True
                    os.path.join(folder, ADAPTER_WEIGHTS[1]))
 
 
-def save_combined_model(model_dir, unet, text_encoder, new_concept_cfg, tokenizer=None):
+UNCHANGED_BY_FUSION = ('vae', 'scheduler')
+
+
+def save_combined_model(model_dir, unet, text_encoder, new_concept_cfg, tokenizer=None, base_model=None):
     """What gradient_fusion.py:810-813 (`pipe.save_pretrained`) leaves on disk for the sampling scripts: unet/,
     text_encoder/, new_concept_cfg.json AND the tokenizer that carries the added `<new{k}>` tokens — without it the
     concept tokens would be BPE-split into ordinary sub-tokens on reload and the learned embedding rows never selected.
-    (The VAE / scheduler folders of the base model are untouched by the fusion; the caller copies them.)"""
+    `base_model`: the directory the fusion started from; those of its vae/ and scheduler/ folders that exist are copied
+    byte for byte (the fusion does not change them), so the fused directory loads as a whole pipeline."""
+    import shutil
     save_unet(unet, model_dir)
     save_text_encoder(text_encoder, model_dir)
     if tokenizer is not None:
         tokenizer.save_pretrained(os.path.join(model_dir, 'tokenizer'))
     with open(os.path.join(model_dir, 'new_concept_cfg.json'), 'w') as f:
         json.dump(new_concept_cfg, f)
+    for sub in UNCHANGED_BY_FUSION:
+        if base_model is not None and os.path.isdir(os.path.join(base_model, sub)):
+            shutil.copytree(os.path.join(base_model, sub), os.path.join(model_dir, sub), dirs_exist_ok=True)
 
 
 def ensure_concept_tokens(tokenizer, new_concept_cfg):

@@ -5,7 +5,9 @@ on `RegionallyT2IAdapterPipeline` (mixofshow/pipelines/pipeline_regionally_t2iad
 Conditions are condition images (`--keypose_condition` / `--sketch_condition`, as in the reference) run through T2I-Adapters
 loaded from LOCAL directories (`--keypose_adapter` / `--sketch_adapter`: the reference downloads them from the hub), or
 pre-computed adapter feature maps (`--keypose_adapter_state` / `--sketch_adapter_state file.pt`: the 4 maps a T2IAdapter
-returns).  Out of scope here (SURVEY.md §8f): the VAE, so the result is written as latents."""
+returns).  Outputs under --save_dir: `latents---<seed>[---<suffix>].pt` and `config.json` always, and, when the model
+directory has `vae/`, the decoded image as the reference names it, `seed_<seed>/<prompt>---<suffix>---<hash8>.png`, with
+its sampling configuration in the `.txt` beside it (image_record)."""
 import argparse
 import ast
 import json
@@ -36,10 +38,16 @@ def prepare_text(prompt, region_prompts, height, width):
     return (prompt, region_collection)
 
 
-def build_model(pretrained_model, device='cuda', tokenizer=None):
-    """reference :55-64: pipeline + new_concept_cfg.json from a fused model directory."""
+def build_model(pretrained_model, device='cuda', tokenizer=None, with_vae=True):
+    """reference :55-64: pipeline + new_concept_cfg.json from a fused model directory, with the scheduler of its
+    `scheduler/` config (DPMSolverPP2M.from_pretrained: the SD1.5 defaults without one; a config the fused step does not
+    compute raises ValueError before anything is loaded) and, when the directory has `vae/` and `with_vae` is set, the
+    GPU VAE.  The VAE is attached after the pipeline is built, so the latent grid stays at 1/8 of the image (the
+    T2I-Adapters' downscale factor) and the latents are the same with or without it, on every rank."""
     from mixofshow.pipelines.pipeline_regionally_t2iadapter import RegionallyT2IAdapterPipeline
     from mixofshow.utils import model_io
+    from mos_b200.scheduler import DPMSolverPP2M
+    scheduler = DPMSolverPP2M.from_pretrained(pretrained_model, subfolder='scheduler')
     assert os.path.exists(os.path.join(pretrained_model, 'new_concept_cfg.json'))
     unet = model_io.load_unet(pretrained_model)
     text_encoder = model_io.load_text_encoder(pretrained_model, device=device)
@@ -48,8 +56,11 @@ def build_model(pretrained_model, device='cuda', tokenizer=None):
         tokenizer = CLIPTokenizer.from_pretrained(pretrained_model, subfolder='tokenizer')
     new_concept_cfg = model_io.load_new_concept_cfg(pretrained_model)
     model_io.ensure_concept_tokens(tokenizer, new_concept_cfg)      # the fused model's added `<new{k}>` tokens
-    pipe = RegionallyT2IAdapterPipeline(text_encoder=text_encoder, tokenizer=tokenizer, unet=unet).to(device)
+    pipe = RegionallyT2IAdapterPipeline(text_encoder=text_encoder, tokenizer=tokenizer, unet=unet,
+                                        scheduler=scheduler).to(device)
     pipe.set_new_concept_cfg(new_concept_cfg)
+    if with_vae and os.path.isdir(os.path.join(pretrained_model, 'vae')):
+        pipe.vae = model_io.load_vae(pretrained_model, device=device)
     return pipe
 
 
@@ -116,7 +127,7 @@ def load_conditions(args):
 def main(argv=None):
     """`python regionally_controlable_sampling.py ...`, or `torchrun --nproc_per_node 2 ...`: the two ranks sample the one
     image together, each running one classifier-free-guidance half (RegionallyT2IAdapterPipeline's `cfg_group`), and
-    rank 0 alone writes the outputs."""
+    rank 0 alone loads the VAE, decodes and writes the outputs."""
     import torch.distributed as dist
     from mos_b200 import dp
     args = parse_args(argv)
@@ -133,8 +144,29 @@ def main(argv=None):
             dist.destroy_process_group()
 
 
+def image_record(args, context_prompt):
+    """Where the reference writes the image and what it records beside it (reference :166-181) -> (lines, name).
+    `lines`: the sampling configuration as 'key: value\\n' lines: pretrained_model, context_prompt, neg_context_prompt,
+    then for sketch and for keypose the condition (the image path as given, or None), adaptor_weight and
+    region_adaptor_weight, then 'random seed' and prompt_rewrite; values are the arguments as passed (str() of each).
+    `name`: 'seed_<seed>/<context prompt, spaces as _>---<suffix>---<hash8>.png' relative to the save directory, hash8
+    being the first 8 hex digits of the SHA-256 of the lines' UTF-8 text.  The lines go to the same name with '.txt'."""
+    import hashlib
+    entries = [('pretrained_model', args.pretrained_model), ('context_prompt', args.prompt),
+               ('neg_context_prompt', args.negative_prompt)]
+    for kind in ('sketch', 'keypose'):
+        entries += [(f'{kind}_condition', getattr(args, f'{kind}_condition')),
+                    (f'{kind}_adaptor_weight', getattr(args, f'{kind}_adaptor_weight')),
+                    (f'region_{kind}_adaptor_weight', getattr(args, f'region_{kind}_adaptor_weight'))]
+    entries += [('random seed', args.seed), ('prompt_rewrite', args.prompt_rewrite)]
+    lines = [f'{key}: {value}\n' for key, value in entries]
+    digest = hashlib.sha256(''.join(lines).encode('utf-8')).hexdigest()[:8]
+    name = f"{context_prompt.replace(' ', '_')}---{args.suffix}---{digest}.png"
+    return lines, os.path.join(f'seed_{args.seed}', name)
+
+
 def _sample(args, conds, rank, device, cfg_group):
-    pipe = build_model(args.pretrained_model, device)
+    pipe = build_model(args.pretrained_model, device, with_vae=rank == 0)
     kwargs = {'height': args.height, 'width': args.width, 'output_type': 'latent', 'cfg_group': cfg_group}
     for kind in ('sketch', 'keypose'):
         path = getattr(args, f'{kind}_adapter_state')
@@ -159,6 +191,15 @@ def _sample(args, conds, rank, device, cfg_group):
         with open(os.path.join(args.save_dir, 'config.json'), 'w') as f:
             json.dump(config, f)
         print(f'save to: {out}')
+        if pipe.vae is not None:
+            from mixofshow.pipelines.pipeline_edlora import decode_latents
+            lines, name = image_record(args, input_prompt[0][0])
+            png = os.path.join(args.save_dir, name)
+            os.makedirs(os.path.dirname(png), exist_ok=True)
+            decode_latents(pipe.vae, latents)[0].save(png)
+            with open(png[:-len('.png')] + '.txt', 'w') as f:
+                f.writelines(lines)
+            print(f'save to: {png}')
     return latents
 
 
