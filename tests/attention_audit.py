@@ -316,13 +316,13 @@ def check_launch(rec):
         pad = nt * QT - n
         e2 = torch.nn.functional.pad((err * err).reshape(got.shape[0], n, -1), (0, 0, 0, pad))
         r2 = torch.nn.functional.pad((ref * ref).reshape(got.shape[0], n, -1), (0, 0, 0, pad))
-        e2 = e2.view(got.shape[0], nt, -1).sum(-1)
+        e2 = e2.reshape(got.shape[0], nt, -1).sum(-1)       # reshape: the window may be a strided view (B = 1)
         if name == 'lse2':                                                  # absolute RMS per tile
             cnt = torch.full((nt,), float(QT), dtype=torch.float64, device=e2.device)
             cnt[-1] = QT - pad
             rel = (e2 / cnt).sqrt()
         else:
-            r2 = r2.view(got.shape[0], nt, -1).sum(-1)
+            r2 = r2.reshape(got.shape[0], nt, -1).sum(-1)
             rel = torch.where(e2 == 0, torch.zeros_like(e2), e2.sqrt() / r2.sqrt())
         rel = rel.nan_to_num(nan=math.inf)
         tol = _tile_tol(rec, name)

@@ -92,9 +92,9 @@ def train_sd15_channels_whole_block(audit, attn_reg_weight=None, optimizer_step=
         _run(audit, eng.optimizer_step, register=[eng.state.params, *eng._lora_keep, *packed])
 
 
-def build_train_sd15_full(use_graph=True):
-    """The training step of bench.py `train_leg` at B = 2 (the shipped configs' batch_size_per_gpu): SD1.5 UNet at 64 x 64
-    with a rank-4 `where: Attention` LoRA, the attention regulariser on all 16 cross layers (weight 0.01,
+def build_train_sd15_full(use_graph=True, B=2):
+    """The training step of bench.py `train_leg` at batch B (2 = the shipped configs' batch_size_per_gpu): SD1.5 UNet at
+    64 x 64 with a rank-4 `where: Attention` LoRA, the attention regulariser on all 16 cross layers (weight 0.01,
     reg_full_identity=False) and a 12-layer CLIPTrainEngine over 16 * B layer-major sequences attached (text_grad), all in
     one shared dp.FlatTrainState.  -> SimpleNamespace(eng, text, state, B, nx, concept_ids)"""
     import math
@@ -105,7 +105,7 @@ def build_train_sd15_full(use_graph=True):
     from mos_b200.train_engine import TrainEngine
     import bench
     sd, lora, _, _, _ = bench.build_workload()
-    B, dev = 2, torch.device('cuda')
+    dev = torch.device('cuda')
     tsd = bench.synthetic_clip_state()
     g0 = torch.Generator().manual_seed(12)
     tlora = {}                                      # the CLIPAttention LoRA train_leg builds
@@ -129,7 +129,9 @@ def build_train_sd15_full(use_graph=True):
 
 def train_sd15_full_inputs(w, seed):
     """one batch of the bench leg's kind: x0, noise, t, box masks and layer-major token ids [16 * B, 77] (BOS, 8 words with
-    the two concept tokens of each layer at positions 2 and 3, EOS padding); the box moves with the seed"""
+    the two concept tokens of each layer at positions 2 and 3, EOS padding); the box moves with the seed.  At B != 2 the
+    prompts have 9 words and sample b carries its concept tokens at positions 1 + b and 3 + 2b, so that they differ
+    per sample"""
     B, nx = w.B, w.nx
     g = torch.Generator().manual_seed(seed)
     x0 = torch.randn(B, 4, 64, 64, generator=g).cuda()
@@ -137,13 +139,15 @@ def train_sd15_full_inputs(w, seed):
     t = torch.randint(0, 1000, (B,), generator=g).cuda()
     ids = torch.randint(1000, 40000, (nx, B, 77), generator=g)
     ids[:, :, 0] = 49406
-    ids[:, :, 9:] = 49407
+    ids[:, :, 9 if B == 2 else 10:] = 49407
+    pos = [[2, 3]] * B if B == 2 else [[1 + b, 3 + 2 * b] for b in range(B)]
     for l in range(nx):
-        ids[l, :, 2], ids[l, :, 3] = w.concept_ids[l % 16], w.concept_ids[16 + l % 16]
+        for b, (p0, p1) in enumerate(pos):
+            ids[l, b, p0], ids[l, b, p1] = w.concept_ids[l % 16], w.concept_ids[16 + l % 16]
     r0, c0 = (int(v) for v in torch.randint(0, 17, (2,), generator=g))
     masks = torch.zeros(B, 1, 64, 64)
     masks[:, :, r0:r0 + 48, c0:c0 + 32] = 1.0
-    return dict(latents=x0, noise=noise, timesteps=t, ehs_layers=None, masks=masks.cuda(), token_pos=[[2, 3]] * B,
+    return dict(latents=x0, noise=noise, timesteps=t, ehs_layers=None, masks=masks.cuda(), token_pos=pos,
                 text_ids=ids.reshape(nx * B, 77))
 
 
@@ -161,11 +165,12 @@ def _packed_lora(ents):
             if isinstance(e.get(k), torch.Tensor)]
 
 
-def train_sd15_full(audit):
-    """bench.py `train_leg` at B = 2, eager: one forward_backward (CLIP forward, UNet forward at 64 x 64, masked MSE, the
+def train_sd15_full(audit, B=2, w=None):
+    """bench.py `train_leg` at batch B, eager: one forward_backward (CLIP forward, UNet forward at 64 x 64, masked MSE, the
     regulariser at 64^2 / 32^2 / 16^2 / 8^2, UNet backward with d(text embeddings), CLIP backward), then the optimiser step
-    (its lora_pack tables point into the flat state and both engines' GEMM operands, registered with the audit)"""
-    w = build_train_sd15_full(use_graph=False)
+    (its lora_pack tables point into the flat state and both engines' GEMM operands, registered with the audit).
+    w: an eager build_train_sd15_full to run on instead of a new one"""
+    w = w or build_train_sd15_full(use_graph=False, B=B)
     batch = train_sd15_full_inputs(w, 100)
     _run(audit, lambda: w.eng.forward_backward(**batch))
     text_ents = [v for ent in w.text.w.values() for v in ent.values()]

@@ -24,7 +24,8 @@ FINETUNE = {'text_embedding': {'enable_tuning': True, 'lr': 1e-3},
             'unet': {'enable_tuning': True, 'lora_cfg': {'rank': 4, 'alpha': 1.0, 'where': 'Attention'}, 'lr': 1e-4}}
 
 
-def _train_one(tmp_path, base, tag, concept_token, init_token, caption, seed):
+def _train_one(tmp_path, base, tag, concept_token, init_token, caption, seed, batch_size_per_gpu=2,
+               gradient_accumulation_steps=1):
     import train_edlora
     g = torch.Generator().manual_seed(seed)
     n = 8
@@ -33,9 +34,9 @@ def _train_one(tmp_path, base, tag, concept_token, init_token, caption, seed):
     data = str(tmp_path / f'{tag}_data.pt')
     torch.save({'latents': torch.randn(n, 4, 32, 32, generator=g) * 0.8, 'prompts': [caption] * n, 'masks': masks}, data)
     out_dir = str(tmp_path / f'{tag}_models')
-    opt = {'name': tag, 'manual_seed': seed, 'gradient_accumulation_steps': 1,
+    opt = {'name': tag, 'manual_seed': seed, 'gradient_accumulation_steps': gradient_accumulation_steps,
            'datasets': {'train': {'path': data, 'replace_mapping': {'<TOK>': concept_token.replace('+', ' ')},
-                                  'batch_size_per_gpu': 2, 'dataset_enlarge_ratio': 1}},
+                                  'batch_size_per_gpu': batch_size_per_gpu, 'dataset_enlarge_ratio': 1}},
            'models': {'pretrained_path': base, 'enable_edlora': True, 'new_concept_token': concept_token,
                       'initializer_token': init_token, 'finetune_cfg': FINETUNE, 'noise_offset': 0.01, 'attn_reg_weight': 0.01,
                       'reg_full_identity': False, 'use_mask_loss': True, 'gradient_checkpoint': False, 'enable_xformers': True,
@@ -46,7 +47,9 @@ def _train_one(tmp_path, base, tag, concept_token, init_token, caption, seed):
     yml = str(tmp_path / f'{tag}.yml')
     yaml.safe_dump(opt, open(yml, 'w'))
     losses = train_edlora.main(['-opt', yml])
-    assert len(losses) == 4 and all(l == l and l > 0 for l in losses)          # 8 samples / batch 2 = 4 optimiser steps
+    steps = train_edlora.total_iterations(n, batch_size_per_gpu, 1, gradient_accumulation_steps)
+    assert len(losses) == steps == n // (batch_size_per_gpu * gradient_accumulation_steps)   # 8 / (2 x 1) = 4 by default
+    assert all(l == l and l > 0 for l in losses)
     ckpt = os.path.join(out_dir, 'edlora_model-latest.pth')
     params = torch.load(ckpt)['params']
     words = concept_token.split('+')

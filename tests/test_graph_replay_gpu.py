@@ -27,12 +27,21 @@ def assert_bits_equal(got, want, what):
 
 
 def test_train_step_graph_matches_eager(cuda):
-    """bench.py's training step at B = 2 (SD1.5 UNet at 64 x 64 + 12-layer CLIP, regulariser, shared flat state), three
+    _train_step_graph_matches_eager(2)
+
+
+def test_train_step_graph_matches_eager_batch4(cuda):
+    """the same at batch_size_per_gpu 4, per-sample concept-token positions"""
+    _train_step_graph_matches_eager(4)
+
+
+def _train_step_graph_matches_eager(B):
+    """bench.py's training step at batch B (SD1.5 UNet at 64 x 64 + 12-layer CLIP, regulariser, shared flat state), three
     steps on different x0 / noise / t / masks / token ids.  In each step the same inputs run eager, then through the captured
     graph (step 1 captures the plain graph, step 2 replays it, step 3 captures the accumulate=True graph), each from the same
     gradient bytes; the loss and the whole flat gradient buffer (with the two logged scalars) must agree bit for bit.
     The bench optimiser step follows, so that every step runs on re-packed LoRA operands."""
-    w = walks.build_train_sd15_full(use_graph=True)
+    w = walks.build_train_sd15_full(use_graph=True, B=B)
     eng, state = w.eng, w.state
     for step, seed in enumerate((200, 201, 202), 1):
         batch = walks.train_sd15_full_inputs(w, seed)

@@ -213,3 +213,55 @@ def test_latent_dataset_and_yml_options(tmp_path):
     assert opt['models']['finetune_cfg']['text_embedding']['lr'] == 1e-3 and opt['train']['emb_norm_threshold'] == 0.55
     params = inspect.signature(EDLoRATrainer.__init__).parameters
     assert all(k in params for k in opt['models']), 'EDLoRATrainer(**opt["models"]) must accept every key of the yml'
+
+
+@pytest.mark.parametrize('batch,world', [(3, 1), (4, 1), (3, 2), (4, 2)])
+def test_latent_dataset_batches_cover_each_epoch(tmp_path, batch, world):
+    """LatentDataset.batches at batch 3 / 4 on 1 / 2 ranks: full batches only (drop_last), and in each epoch the ranks'
+    slices are disjoint and together are the epoch's permutation less its remainder, step by step in order"""
+    import train_edlora as te
+    n = 13
+    torch.save({'latents': torch.arange(n, dtype=torch.float32).view(n, 1, 1, 1).expand(n, 4, 2, 2).clone(),
+                'prompts': [f'p{i}' for i in range(n)], 'masks': torch.ones(n, 1, 2, 2)}, str(tmp_path / 'set.pt'))
+    ds = te.LatentDataset({'path': str(tmp_path / 'set.pt')})
+    its = [ds.batches(batch, rank=r, world=world, seed=3) for r in range(world)]
+    g = torch.Generator().manual_seed(3)
+    steps = n // (batch * world)
+    for _ in range(2):                                       # two epochs: the second permutation follows the first
+        perm = torch.randperm(n, generator=g).tolist()
+        got = []
+        for _ in range(steps):
+            for it in its:
+                b = next(it)
+                idx = [int(x) for x in b['images'][:, 0, 0, 0]]
+                assert len(idx) == batch and b['prompts'] == [f'p{i}' for i in idx]
+                got += idx
+        assert got == perm[:steps * batch * world]
+        assert len(set(got)) == len(got)
+
+
+def test_layerwise_tokens_and_concept_positions_at_batch_3():
+    """EDLoRATrainer.tokenize_layerwise at b = 3: the layer-major ids are ids_lm[l * b + i] == ids[i * 16 + l]; and
+    concept_token_positions finds each sample's own positions"""
+    from test_fusion_orchestration import WordTokenizer
+    from mixofshow.pipelines.trainer_edlora import EDLoRATrainer
+    from types import SimpleNamespace
+    tok = WordTokenizer()
+    names = [f'<new{i}>' for i in range(32)]
+    tok.add_tokens(names)
+    cfg = {'<c1>': {'concept_token_names': names[:16], 'concept_token_ids': list(range(49408, 49424))},
+           '<c2>': {'concept_token_names': names[16:], 'concept_token_ids': list(range(49424, 49440))}}
+    tr = SimpleNamespace(new_concept_cfg=cfg, tokenizer=tok,
+                         get_all_concept_token_ids=lambda: list(range(49408, 49440)))
+    prompts = ['<c1> <c2> walking', 'a photo of <c1> <c2>', 'the <c1> in a red <c2> hat']
+    ids, ids_lm = EDLoRATrainer.tokenize_layerwise(tr, prompts)
+    b = 3
+    assert ids.shape == (16 * b, 77) and ids_lm.shape == (16 * b, 77)
+    for l in range(16):
+        for i in range(b):
+            assert torch.equal(ids_lm[l * b + i], ids[i * 16 + l])
+            assert int(ids[i * 16 + l][[1, 4, 2][i]]) == 49408 + l      # layer l reads its own concept token
+    pos = EDLoRATrainer.concept_token_positions(tr, ids, b)
+    assert pos == [[1, 2], [4, 5], [2, 6]]
+    from oracle import train_ref
+    assert train_ref.concept_token_positions(ids, b, tr.get_all_concept_token_ids()) == pos

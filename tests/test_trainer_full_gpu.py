@@ -2,7 +2,10 @@
 prompts -> bind_concept_prompt -> tokenizer -> CLIP text encoder (LoRA) -> UNet (LoRA) -> masked MSE + attention regulariser
 -> backward through BOTH networks, against fp32 autograd through transformers' CLIPTextModel chained into the oracle UNet
 (reference LoRA formula injected in both, oracle/train_ref.py loss).  Checks the three parameter groups of
-trainer_edlora.py:82-139: new-concept embedding rows, CLIPAttention LoRA, UNet Attention LoRA.
+trainer_edlora.py:82-139: new-concept embedding rows, CLIPAttention LoRA, UNet Attention LoRA.  At B = 1, 2, 3 and 4 with
+both regulariser modes: much of the step depends on B (the loss's 1 / B, the regulariser's batch-wide maxima and zero
+count, the GroupNorm partitions, the split-K and row blocking of M = B x HW, the 16 x B text sequences), and the samples of
+a batch differ in prompt length, timestep and mask, so that a sample mix-up shows.
 
 Tolerances: bf16 operands through two networks forward and backward: whole-group gradient rel-L2 <= 4e-2, cosine >= 0.998;
 loss within 2 %."""
@@ -47,39 +50,51 @@ def _base_dir(tmp_path, clip_layers=2):
     return base, ref_unet, clip
 
 
-def test_full_trainer_step_vs_autograd(cuda, tmp_path):
-    from test_fusion_orchestration import WordTokenizer
-    from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt
-    from mixofshow.pipelines.trainer_edlora import EDLoRATrainer
-    from mixofshow.utils.ptp_util import AttentionStore
-    from oracle import inject, train_ref
-    from oracle.schedulers import DDPMScheduler
-    base, ref_unet, clip = _base_dir(tmp_path)
-    tok = WordTokenizer()
-    reg_w = 0.05
-    tr = EDLoRATrainer(base, '<c1>+<c2>', '<rand-0.02>+<rand-0.02>', True, finetune_cfg=json.loads(json.dumps(FINETUNE)),
-                       noise_offset=None, attn_reg_weight=reg_w, reg_full_identity=False, use_mask_loss=True,
-                       enable_xformers=True, tokenizer=tok, latent_size=(16, 16))
-    assert tr.new_concept_cfg['<c2>']['concept_token_names'] == [f'<new{16 + i}>' for i in range(16)]
-    ids_concept = tr.get_all_concept_token_ids()
-    assert ids_concept == list(range(49408, 49408 + 32))
-    g = torch.Generator().manual_seed(5)
-    delta = {'new_concept_embedding': {'<c1>': torch.randn(16, 768, generator=g) * 0.02,
-                                       '<c2>': torch.randn(16, 768, generator=g) * 0.02},
-             'text_encoder': inject.random_lora_state(clip, seed=3, where='CLIPAttention', up_std=0.05),
-             'unet': inject.random_lora_state(ref_unet, seed=10)}
-    tr.load_delta_state_dict(delta)
-    B, H = 2, 16
-    prompts = ['photo of a <c1> <c2>', 'the <c1> <c2> on a beach']
-    lat = torch.randn(B, 4, H, H, generator=g)
-    noise = torch.randn(B, 4, H, H, generator=g)
-    t = torch.tensor([130, 811])
+PREFIX = ('photo of a', 'the', 'a close photo of one', 'an old')     # sample b's concept words sit at a position of its own
+SUFFIX = ('', 'on a beach', 'smiling', 'in the snow')
+
+
+def batch_inputs(B, seed, words=('<c1>', '<c2>'), H=16):
+    """a training batch whose samples differ where the step could mix them up: prompt length (so the concept-token
+    positions), timestep (0 and 999 among them), mask; at B >= 2 the last mask is all ones, so that sample adds to the
+    regulariser's zero-pixel count only through the others.  -> prompts, latents, noise, timesteps, masks"""
+    g = torch.Generator().manual_seed(seed)
+    prompts = [f'{PREFIX[b]} {words[0]} {words[1]} {SUFFIX[b]}'.strip() for b in range(B)]
+    lat, noise = torch.randn(B, 4, H, H, generator=g), torch.randn(B, 4, H, H, generator=g)
+    t = torch.tensor([0, 999, 511, 130][:B])
     masks = (torch.rand(B, 1, H, H, generator=g) > 0.5).float()
     masks[:, :, 4:9, 4:9] = 1.0
     masks[:, :, 0, 0] = 0.0
-    loss = tr(lat, prompts, masks, torch.ones_like(masks), noise=noise, timesteps=t)
-    torch.cuda.synchronize()
-    # ---------------- reference chain in fp32 autograd
+    if B >= 2:
+        masks[B - 1] = 1.0
+    return prompts, lat, noise, t, masks
+
+
+def _trainer(base, tok, reg_w, full):
+    from mixofshow.pipelines.trainer_edlora import EDLoRATrainer
+    return EDLoRATrainer(base, '<c1>+<c2>', '<rand-0.02>+<rand-0.02>', True, finetune_cfg=json.loads(json.dumps(FINETUNE)),
+                         noise_offset=None, attn_reg_weight=reg_w, reg_full_identity=full, use_mask_loss=True,
+                         enable_xformers=True, tokenizer=tok, latent_size=(16, 16))
+
+
+def _delta(ref_unet, clip):
+    from oracle import inject
+    g = torch.Generator().manual_seed(5)
+    return {'new_concept_embedding': {'<c1>': torch.randn(16, 768, generator=g) * 0.02,
+                                      '<c2>': torch.randn(16, 768, generator=g) * 0.02},
+            'text_encoder': inject.random_lora_state(clip, seed=3, where='CLIPAttention', up_std=0.05),
+            'unet': inject.random_lora_state(ref_unet, seed=10)}
+
+
+def autograd_reference(tr, clip, ref_unet, delta, tok, batches, reg_w, full):
+    """the step in fp32 autograd: transformers' CLIPTextModel chained into the oracle UNet, reference LoRA formula injected
+    in both, oracle/train_ref.py loss.  The gradients of all `batches` ((prompts, latents, noise, t, masks) each, one
+    backward per batch, the regulariser per batch as the reference computes it) are summed.
+    -> (losses, d concept rows [32, 768], text LoRA leaves, UNet LoRA leaves); the leaves hold the gradients"""
+    from mixofshow.pipelines.pipeline_edlora import bind_concept_prompt
+    from mixofshow.utils.ptp_util import AttentionStore
+    from oracle import inject, train_ref
+    from oracle.schedulers import DDPMScheduler
     clip.resize_token_embeddings(49408 + 32)
     emb = clip.get_input_embeddings().weight
     with torch.no_grad():
@@ -91,22 +106,26 @@ def test_full_trainer_step_vs_autograd(cuda, tmp_path):
     inject.inject_lora(clip, t_leaves, 1.0)
     inject.inject_lora(ref_unet, u_leaves, 1.0)
     ctl = AttentionStore(training=True)
-    n_x = inject.install_control_processors(ref_unet, ctl)
-    ids = tok(bind_concept_prompt(prompts, tr.new_concept_cfg), padding='max_length', max_length=77,
-              return_tensors='pt').input_ids
-    ehs = clip(ids)[0].view(B, 16, 77, 768)
-    pos = train_ref.concept_token_positions(ids, B, ids_concept)
-    noisy = DDPMScheduler().add_noise(lat, noise, t)
-    loss_ref, _, _ = train_ref.train_loss(ref_unet, ctl, noisy, t, ehs, noise, masks, masks, pos, reg_full_identity=False,
-                                          attn_reg_weight=reg_w)
-    loss_ref.backward()
-    print(f'full trainer step: loss {loss.item():.6f} vs autograd {loss_ref.item():.6f}  ({n_x} cross-attention layers)')
-    assert abs(loss.item() - loss_ref.item()) < 2e-2 * abs(loss_ref.item())
-    # group 0: embedding rows
-    g_emb_ref = emb.grad[49408:49408 + 32]
-    e0, c0 = rel_l2(tr.text_engine.emb_grad, g_emb_ref), _cos(tr.text_engine.emb_grad, g_emb_ref)
-    # group 1: text LoRA, group 2: UNet LoRA
-    res = {}
+    inject.install_control_processors(ref_unet, ctl)
+    losses = []
+    for prompts, lat, noise, t, masks in batches:
+        b = len(prompts)
+        ids = tok(bind_concept_prompt(prompts, tr.new_concept_cfg), padding='max_length', max_length=77,
+                  return_tensors='pt').input_ids
+        ehs = clip(ids)[0].view(b, 16, 77, 768)
+        pos = train_ref.concept_token_positions(ids, b, tr.get_all_concept_token_ids())
+        noisy = DDPMScheduler().add_noise(lat, noise, t)
+        loss_ref, _, _ = train_ref.train_loss(ref_unet, ctl, noisy, t, ehs, noise, masks, masks, pos,
+                                              reg_full_identity=full, attn_reg_weight=reg_w)
+        loss_ref.backward()
+        losses.append(loss_ref.item())
+        ctl.reset()
+    return losses, emb.grad[49408:49408 + 32], t_leaves, u_leaves
+
+
+def group_errors(tr, g_rows, t_leaves, u_leaves):
+    """{'rows' | 'text' | 'unet': (rel-L2, cosine, size)} of the trainer's gradient against autograd's"""
+    res = {'rows': (rel_l2(tr.text_engine.emb_grad, g_rows), _cos(tr.text_engine.emb_grad, g_rows), g_rows.numel())}
     for name, eng, leaves in (('text', tr.text_engine, t_leaves), ('unet', tr.engine, u_leaves)):
         fg, fr = [], []
         for m, (gd, gu) in eng.lora_grad_dict().items():
@@ -115,11 +134,53 @@ def test_full_trainer_step_vs_autograd(cuda, tmp_path):
                    leaves[m + '.lora_up.weight'].grad.reshape(gu.shape).flatten()]
         fg, fr = torch.cat(fg), torch.cat(fr)
         res[name] = (rel_l2(fg, fr), _cos(fg, fr), fg.numel())
-    print(f'  embedding rows: rel-L2 {e0:.3e} cos {c0:.5f};  text LoRA ({res["text"][2]}): rel-L2 {res["text"][0]:.3e} cos '
-          f'{res["text"][1]:.5f};  unet LoRA ({res["unet"][2]}): rel-L2 {res["unet"][0]:.3e} cos {res["unet"][1]:.5f}')
-    assert e0 < 4e-2 and c0 > 0.998
-    for name in ('text', 'unet'):
-        assert res[name][0] < 4e-2 and res[name][1] > 0.998
+    return res
+
+
+def format_errors(res):
+    return ';  '.join(f'{name} ({n}): rel-L2 {r:.3e} cos {c:.5f}' for name, (r, c, n) in res.items())
+
+
+def test_full_trainer_step_vs_autograd(cuda, tmp_path):
+    """the shipped batch, B = 2, regulariser with reg_full_identity=False"""
+    _full_trainer_step_vs_autograd(tmp_path, 2, False)
+
+
+# the other batch sizes and regulariser modes (the B = 2 / reg_full_identity=False case is the test above)
+BATCH_CASES = [(b, f) for b in (1, 2, 3, 4) for f in (False, True) if (b, f) != (2, False)]
+
+
+@pytest.mark.parametrize('B,full', BATCH_CASES,
+                         ids=[f'B{b}-{"reg_full_identity" if f else "reg_subject_outside"}' for b, f in BATCH_CASES])
+def test_full_trainer_step_vs_autograd_batch(cuda, tmp_path, B, full):
+    _full_trainer_step_vs_autograd(tmp_path, B, full)
+
+
+def _full_trainer_step_vs_autograd(tmp_path, B, full):
+    from test_fusion_orchestration import WordTokenizer
+    base, ref_unet, clip = _base_dir(tmp_path)
+    tok = WordTokenizer()
+    reg_w = 0.05
+    tr = _trainer(base, tok, reg_w, full)
+    assert tr.new_concept_cfg['<c2>']['concept_token_names'] == [f'<new{16 + i}>' for i in range(16)]
+    assert tr.get_all_concept_token_ids() == list(range(49408, 49408 + 32))
+    delta = _delta(ref_unet, clip)
+    tr.load_delta_state_dict(delta)
+    prompts, lat, noise, t, masks = batch_inputs(B, seed=40 + B)
+    loss = tr(lat, prompts, masks, torch.ones_like(masks), noise=noise, timesteps=t)
+    torch.cuda.synchronize()
+    assert tr.text_engine.n_seq == len(tr.engine.xattn_names) * B
+    ids, _ = tr.tokenize_layerwise(prompts)
+    pos = tr.concept_token_positions(ids, B)
+    assert len({tuple(p) for p in pos}) == B, pos               # every sample has its concept tokens elsewhere
+    (loss_ref,), g_rows, t_leaves, u_leaves = autograd_reference(tr, clip, ref_unet, delta, tok,
+                                                                 [(prompts, lat, noise, t, masks)], reg_w, full)
+    res = group_errors(tr, g_rows, t_leaves, u_leaves)
+    print(f'full trainer step B={B} full_identity={full}: loss {loss.item():.6f} vs autograd {loss_ref:.6f};  '
+          + format_errors(res))
+    assert abs(loss.item() - loss_ref) < 2e-2 * abs(loss_ref)
+    for name, (r, c, _) in res.items():
+        assert r < 4e-2 and c > 0.998, name
     # checkpoint layout of the reference (trainer_edlora.py:358-378) and round trip
     d = tr.delta_state_dict()
     assert set(d) == {'new_concept_embedding', 'text_encoder', 'unet'} and set(d['new_concept_embedding']) == {'<c1>', '<c2>'}

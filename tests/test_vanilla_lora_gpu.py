@@ -20,7 +20,7 @@ import torch
 import yaml
 
 from test_finetune_groups import COMBOS, combo_id, finetune_cfg
-from test_trainer_full_gpu import _base_dir, _cos, rel_l2
+from test_trainer_full_gpu import _base_dir, _cos, batch_inputs, rel_l2
 
 pytestmark = pytest.mark.gpu
 
@@ -36,7 +36,8 @@ def _trainer(base, combo, tok=None, latent=16):
                          tokenizer=tok or WordTokenizer(), latent_size=(latent, latent))
 
 
-def _data(ref_unet, clip, combo):
+def _data(ref_unet, clip, combo, B=2):
+    """-> delta, prompts, latents, noise, timesteps, masks; at B != 2 the per-sample batch of test_trainer_full_gpu"""
     from oracle import inject
     g = torch.Generator().manual_seed(5)
     d = {'new_concept_embedding': {c: torch.randn(1, 768, generator=g) * 0.02 for c in ('<c1>', '<c2>')},
@@ -45,16 +46,24 @@ def _data(ref_unet, clip, combo):
         d['text_encoder'] = inject.random_lora_state(clip, seed=3, where='CLIPAttention', up_std=0.05)
     if combo[2]:
         d['unet'] = inject.random_lora_state(ref_unet, seed=10)
-    B, H = 2, 16
+    if B != 2:
+        return (d, *batch_inputs(B, seed=50 + B, words=('<new0>', '<new1>')))
+    H = 16
     lat, noise = torch.randn(B, 4, H, H, generator=g), torch.randn(B, 4, H, H, generator=g)
     masks = (torch.rand(B, 1, H, H, generator=g) > 0.5).float()
     masks[:, :, 4:9, 4:9] = 1.0
     masks[:, :, 0, 0] = 0.0
-    return d, lat, noise, torch.tensor([130, 811]), masks
+    return d, PROMPTS, lat, noise, torch.tensor([130, 811]), masks
 
 
-@pytest.mark.parametrize('combo', COMBOS, ids=combo_id)
-def test_vanilla_step_vs_autograd(cuda, tmp_path, combo):
+ALL_GROUPS = (True, True, True)
+# every group subset at B = 2, and all three groups at the other batch sizes (the B = 2 ids stay the combo's)
+STEP_CASES = [(2, c) for c in COMBOS] + [(b, ALL_GROUPS) for b in (1, 3, 4)]
+
+
+@pytest.mark.parametrize('B,combo', STEP_CASES,
+                         ids=[combo_id(c) if b == 2 else f'{combo_id(c)}-B{b}' for b, c in STEP_CASES])
+def test_vanilla_step_vs_autograd(cuda, tmp_path, B, combo):
     from test_fusion_orchestration import WordTokenizer
     from mixofshow.utils.ptp_util import AttentionStore
     from oracle import inject, train_ref
@@ -64,11 +73,11 @@ def test_vanilla_step_vs_autograd(cuda, tmp_path, combo):
     tok = WordTokenizer()
     tr = _trainer(base, combo, tok)
     assert tr.get_all_concept_token_ids() == [49408, 49409]
-    delta, lat, noise, t, masks = _data(ref_unet, clip, combo)
+    delta, prompts, lat, noise, t, masks = _data(ref_unet, clip, combo, B)
     tr.load_delta_state_dict(delta)
-    loss = tr(lat, PROMPTS, masks, torch.ones_like(masks), noise=noise, timesteps=t)    # warm-up + capture + replay
+    loss = tr(lat, prompts, masks, torch.ones_like(masks), noise=noise, timesteps=t)    # warm-up + capture + replay
     torch.cuda.synchronize()
-    assert tr.text_engine.n_seq == 2 and tuple(tr.engine.in_ehs.shape) == (1, 2, 77, 768)
+    assert tr.text_engine.n_seq == B and tuple(tr.engine.in_ehs.shape) == (1, B, 77, 768)
     assert tr.state.grads.numel() == sum(tr.flat_group_sizes()) + 2 and tr.flat_group_sizes()[0] == (2 * 768 if emb_on else 0)
     clip.resize_token_embeddings(49408 + 2)
     emb = clip.get_input_embeddings().weight
@@ -84,9 +93,9 @@ def test_vanilla_step_vs_autograd(cuda, tmp_path, combo):
         inject.inject_lora(clip, t_leaves, 1.0)
     if u_leaves:
         inject.inject_lora(ref_unet, u_leaves, 1.0)
-    ids = tok(PROMPTS, padding='max_length', max_length=77, return_tensors='pt').input_ids       # unbound, [b, 77]
-    assert torch.equal(ids, tr.tokenize(PROMPTS))
-    pos = train_ref.concept_token_positions(ids, 2, tr.get_all_concept_token_ids())
+    ids = tok(prompts, padding='max_length', max_length=77, return_tensors='pt').input_ids       # unbound, [b, 77]
+    assert torch.equal(ids, tr.tokenize(prompts))
+    pos = train_ref.concept_token_positions(ids, B, tr.get_all_concept_token_ids())
     noisy = DDPMScheduler().add_noise(lat, noise, t)
     ours, order = {}, {}
     if emb_on:
@@ -118,7 +127,7 @@ def test_vanilla_step_vs_autograd(cuda, tmp_path, combo):
 
     loss_bf, g_bf = autograd(True)
     loss_ref, g_ref = autograd(False)
-    msg = [f'{combo_id(combo)}: loss {loss.item():.6f} vs {loss_ref:.6f}']
+    msg = [f'{combo_id(combo)} B={B}: loss {loss.item():.6f} vs {loss_ref:.6f}']
     assert abs(loss.item() - loss_ref) < 2e-2 * abs(loss_ref)
     for name, g in ours.items():
         r, c = rel_l2(g, g_ref[name]), _cos(g, g_ref[name])
